@@ -1,4 +1,4 @@
-"""Builds libdistrifuser_b200.so (hand-written sm_100a CUDA behind the C ABI of include/distrifuser_b200.h).
+"""Builds libdistrifuser_b200.so (hand-written sm_90a CUDA behind the C ABI of include/distrifuser_b200.h).
 
 In-tree build so the .so travels with the repo snapshot to the GPU box; nvcc cross-compiles without a GPU."""
 from __future__ import annotations
@@ -11,7 +11,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libdistrifuser_b200.so")
 SOURCES = ("comm.cu", "groupnorm.cu", "halo.cu", "attention.cu", "elementwise.cu", "linear.cu")
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
          "-Xcompiler", "-fPIC", "-shared"]
 
 

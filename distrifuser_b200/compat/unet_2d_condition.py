@@ -69,7 +69,7 @@ class GEGLU(nn.Module):
         self.norm_fused = None        # set by BasicTransformerBlock: LayerNorm whose output feeds this projection (unused here)
 
     def _fused_weights(self, block):
-        """Interleaved copy of proj.weight / proj.bias for the fused tcgen05 GEMM + GEGLU epilogue (ops.linear_geglu); rebuilt
+        """Interleaved copy of proj.weight / proj.bias for the fused wgmma GEMM + GEGLU epilogue (ops.linear_geglu); rebuilt
         when the source tensors change (load_state_dict, .to(), in-place edits) or the kernel wants another block size."""
         from .. import ops
         w, b = self.proj.weight, self.proj.bias

@@ -1,27 +1,23 @@
-// distrifuser_b200 -- fused multi-head attention over per-rank K/V segments (sm_100a: tcgen05 + TMEM + TMA).
+// distrifuser_b200 -- fused multi-head attention over per-rank K/V segments (sm_90a: wgmma + TMA + mbarrier).
 //
 // Replaces, for DistriSelfAttentionPP._forward (distrifuser/modules/pp/attn.py:127-153):
 //     torch.cat(full_kv) over ranks  -> the K/V tiles are TMA-loaded straight from the n per-rank segments
 //                                       (own fresh projection + peers' 1-step-stale arena slots)
 //     torch.split + view/transpose   -> tensor-map coordinates (head, row) select K at column h*d, V at C + h*d
-//     F.scaled_dot_product_attention -> S = Q K^T and O += P V as tcgen05.mma tiles, accumulators in TMEM
+//     F.scaled_dot_product_attention -> S = Q K^T and O += P V as wgmma tiles, accumulators in registers
 // and the SDPA of DistriCrossAttentionPP.forward (attn.py:79-87) with nseg = 1, lseg = 77.
 //
-// Persistent CTAs (384 threads = 3 warpgroups, TWO per SM at d <= 64: 256 TMEM columns, ~97 KB smem each; setmaxnreg moves
-// registers from the producer warpgroup to the two softmax warpgroups) walk work units = one 128-row Q tile of one (batch, head):
-//   warps 0-7  softmax: warp w owns 16 rows and all 128 S columns of them in the 16x256b TMEM fragment layout (a row lives in
-//              one quad).  tcgen05.ld S (S is released at once) -> exp2 in place (packed FFMA2/FADD2, 3 of 16 column groups on a
-//              polynomial instead of MUFU) against a SPECULATIVE exponent reference -- row maxima are only computed for the
-//              first tile of an item; a later tile whose row sums show the reference was too small is repaired in registers
-//              (power-of-two rescale of P, l, O), and an item whose exponentials overflowed fp32 is re-run exactly -- then
-//              P -> fp16 -> TMEM, epilogue O / l -> HBM (or fp32 partials merged by the last part of a split unit)
+// Persistent CTAs (288 threads: two consumer warpgroups + one producer warp; one CTA per SM)
+// walk work items = one 128-row Q tile of one (batch, head), or a K/V range of one:
+//   warps 0-7  two consumer warpgroups, 64 Q rows each.  Per K/V tile: S = Q K^T (m64nSNk16 wgmmas, both operands in shared
+//              memory) into SN/2 fp32 registers per thread, online softmax on that fragment (a row lives in one quad: row maxima
+//              and sums are two shuffles; exp2 on MUFU with 3 of 16 column groups on a polynomial on the FMA pipe; the exponent
+//              reference only moves when the row maximum grew by more than 2^8), P packed to fp16 IN REGISTERS as the A operand of
+//              O += P V (m64n64k16 wgmmas, V MN-major from shared memory), O in registers; epilogue O / l -> HBM (or fp32
+//              partials merged by the last part of a split unit)
 //   warp 8     scheduler + TMA producer: hands out work items through a two-entry ring (whole units drawn from an atomic ticket
-//              counter when the grid fills the SMs, a static one-item list otherwise, replays first), then Q per item and
-//              K (3 stages) / V (2 stages) tiles through mbarrier rings; waits the peers' flags
-//   warp 9     MMA issuer (one lane): S = Q K_j^T (SS), O += P V_j (A = P from TMEM, B = V MN-major); Q K_{j+1}^T is
-//              issued once the softmax warps have released S_j (s_free)
-//   warps 10-11 idle (they complete the third warpgroup: setmaxnreg works on whole warpgroups)
-// TMEM columns: S [0,128) P [128,192) O [192, 192 + 64*NBLK)   (fp32 S/O, packed fp16 P)
+//              counter when the grid fills the SMs, a static one-item list otherwise), then Q per item and K (KST stages) /
+//              V (VST stages) tiles through mbarrier rings; waits the peers' flags
 
 #include "tc_ptx.cuh"
 
@@ -30,51 +26,33 @@ using namespace df::tc;
 
 namespace {
 
-constexpr int BM = 128;      // Q rows per CTA
+constexpr int BM = 128;      // Q rows per CTA (64 per consumer warpgroup)
 constexpr int BN = 128;      // K/V rows per tile
 constexpr int HB = 64;       // head-dim block: one 128-byte swizzled row; d is padded to NBLK * 64 columns (TMA zero-fills)
-constexpr int NSOFTMAX_WARPS = 8;
-#ifndef DF_FMHA_SETMAXNREG
-#define DF_FMHA_SETMAXNREG 1
-#endif
-constexpr int NTHREADS = 32 * (NSOFTMAX_WARPS + (DF_FMHA_SETMAXNREG ? 4 : 2));   // 3 warpgroups: 2 x softmax, 1 x (TMA warp, MMA warp, two idle warps) -- whole
-                                                      // warpgroups so that setmaxnreg may move registers between them
-constexpr int WARP_TMA = NSOFTMAX_WARPS, WARP_MMA = NSOFTMAX_WARPS + 1;
-constexpr uint32_t COL_S = 0, COL_P = 128, COL_O = 192;   // S fp32 [0,128), P packed fp16 [128,192), O fp32 [192, 192 + 64*NBLK)
+constexpr int NCONSUMER_WARPS = 8;
+constexpr int NTHREADS = 32 * (NCONSUMER_WARPS + 1);
+constexpr int WARP_TMA = NCONSUMER_WARPS;
 constexpr uint32_t BLK_BYTES = BN * HB * 2;                // one 128 x 64 fp16 block = 16 KiB
 
-// NBLK = ceil(d / 64): 1 for d in {40, 64} (SDXL, SD1.x level 0: two CTAs per SM), 2 for d = 80, 3 for d = 160 (SD1.x)
+// NBLK = ceil(d / 64): 1 for d in {40, 64} (SDXL, SD1.x level 0), 2 for d = 80, 3 for d = 160 (SD1.x)
 template <int NBLK, int KSTAGES, int VSTAGES>
 struct __align__(1024) SmemT {
   __half q[NBLK][BM * HB];
   __half k[KSTAGES][NBLK][BN * HB];
   __half v[VSTAGES][NBLK][BN * HB];
-  float red_sum[2][BM];      // [unit parity][row]: row sums for the epilogue
-  float red_ref[2][BM];      // [unit parity][row]: exponent reference of every row (log2 units) for the epilogue / split-KV partials
-  uint64_t q_full, q_empty;   // Q tile of the current work unit loaded / no longer read by the tensor core
+  uint64_t q_full, q_empty;   // Q tile of the current work item loaded / no longer read by the tensor cores
   uint64_t k_full[KSTAGES], k_empty[KSTAGES], v_full[VSTAGES], v_empty[VSTAGES];
-  uint64_t s_full;
-  uint64_t s_free;
-  uint64_t p_full;
-  uint64_t pv_done;
-  uint64_t o_free;            // the epilogue of the previous work unit has pulled O out of TMEM
-  uint64_t sched_full[2];     // work-item ring: the TMA lane (scheduler) publishes the next item code, the other roles consume it
+  uint64_t sched_full[2];     // work-item ring: the TMA lane (scheduler) publishes the next item code, the consumers read it
   int sched_code[2];
-  uint32_t replay_code[8];    // items whose speculative pass overflowed fp32 (softmax thread 0 -> scheduler), re-run exactly
-  uint32_t replay_wr;
-  uint32_t items_done;        // items whose verdict (clean / replay) has been published by the softmax warps
-  int poison[4];              // [item & 3]: set by any softmax warp that had to give up on the item
-  uint32_t tmem_base;
   uint32_t ticket;            // arrival ticket of this part among the parts of its left-over unit
 };
+// One CTA per SM.  Registers of a kernel that issues wgmma are allocated per warpgroup, so the producer warp costs a whole
+// warpgroup's share and a thread gets at most 168 (65536 / 384): the S slice (SN / 2), the O fragment (32 per head block) and
+// the packed P (SN / 4) must fit in that -- hence 128-wide S slices at d <= 64 and 64-wide ones for the wider heads.
 template <int NBLK> struct Cfg;
-template <> struct Cfg<1> { static constexpr int KST = 3, VST = 2, CTAS = 2; static constexpr uint32_t TMEM = 256; };
-// Two CTAs of 384 threads per SM start at 80 registers per thread (65536 / 768).  The producer warpgroup gives registers back
-// (setmaxnreg.dec 32) and the two softmax warpgroups take them (setmaxnreg.inc 104: 256 x 104 + 128 x 32 = 384 x 80): the softmax
-// loop holds a 64-value S fragment per thread and ran with spills at the 96 registers an even split allows.
-constexpr int REGS_PRODUCER = 32, REGS_SOFTMAX = 104;   // (10 warps with 112 / 32 -- a partial third warpgroup -- fails at launch: profiles/r2_attn_sweep_setmaxnreg_variants.txt)
-template <> struct Cfg<2> { static constexpr int KST = 2, VST = 2, CTAS = 1; static constexpr uint32_t TMEM = 512; };
-template <> struct Cfg<3> { static constexpr int KST = 2, VST = 1, CTAS = 1; static constexpr uint32_t TMEM = 512; };
+template <> struct Cfg<1> { static constexpr int KST = 3, VST = 2, SN = 128; };
+template <> struct Cfg<2> { static constexpr int KST = 2, VST = 2, SN = 64; };
+template <> struct Cfg<3> { static constexpr int KST = 2, VST = 1, SN = 64; };
 
 // work schedule of one launch (host: plan_schedule): every CTA takes `a` whole units; the R left-over units are cut into P parts
 struct Sched {
@@ -82,7 +60,7 @@ struct Sched {
   int dyn;      // 1: whole units are handed out by an atomic ticket counter (grids that fill the SMs); 0: static list per CTA
   int units;
 };
-constexpr int ITEM_END = -1, ITEM_EXACT = 1 << 30, ITEM_MASK = ITEM_EXACT - 1;
+constexpr int ITEM_END = -1;
 
 __device__ __forceinline__ float2 ld_f2(const float2* p) {          // coherent load (partials were written during this launch)
   float2 r;
@@ -90,44 +68,30 @@ __device__ __forceinline__ float2 ld_f2(const float2* p) {          // coherent 
   return r;
 }
 
-// Scheduler <-> softmax signalling words in shared memory (replay ring, verdict counter) are accessed with shared-memory
-// atomics only: one writer, one polling reader, ordered by __threadfence_block -- no barrier involved, so plain or volatile
-// accesses would be (benign) races in the eyes of the memory model and of compute-sanitizer's racecheck.
-__device__ __forceinline__ uint32_t sig_load(uint32_t* p) { return atomicAdd(p, 0u); }
-__device__ __forceinline__ void sig_store(uint32_t* p, uint32_t v) { atomicExch(p, v); }
-
 struct SegInfo {
   int32_t rank[DF_MAX_WORLD];  // world rank holding segment s
 };
 
-#ifndef DF_OPAQUE_BASES
-#define DF_OPAQUE_BASES 1
-#endif
 #ifndef DF_EMU_GROUPS
 #define DF_EMU_GROUPS 3      // of the 16 column groups of a tile row, this many (evenly spread) take the polynomial exp2 (FMA/ALU
 #endif                       // pipes) instead of MUFU
 
-#ifdef DF_TRACE
-// cycle-level event trace of CTA (0,0,0) for kernel tuning (tools/trace_attn.py); compiled out by default
-__device__ long long df_trace_buf[64 * 16];
-#define DF_TR(slot, tile) do { if (blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0 && (tile) < 64) df_trace_buf[(tile) * 16 + (slot)] = clock64(); } while (0)
-#else
-#define DF_TR(slot, tile) do {} while (0)
-#endif
-
-// instruction descriptors (kind::f16, fp16 inputs, fp32 accumulate, M = 128)
-constexpr uint32_t IDESC_S = (1u << 4) | ((uint32_t)(BN >> 3) << 17) | ((uint32_t)(BM >> 4) << 24);               // K-major A, K-major B
-constexpr uint32_t IDESC_PV = (1u << 4) | (1u << 16) | ((uint32_t)(HB >> 3) << 17) | ((uint32_t)(BM >> 4) << 24);  // B (=V) MN-major, N = 64
+template <int N>
+__device__ __forceinline__ void wgmma_ss(float* d, uint64_t a_desc, uint64_t b_desc, uint32_t accumulate) {
+  if constexpr (N == 64) wgmma_ss_n64(d, a_desc, b_desc, accumulate);
+  else wgmma_ss_n128(d, a_desc, b_desc, accumulate);
+}
 
 // ----------------------------------------------------------------------------------------- kernel
 template <int NBLK>
-__global__ void __launch_bounds__(NTHREADS, Cfg<NBLK>::CTAS)
+__global__ void __launch_bounds__(NTHREADS, 1)
 fmha_fwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant__ CUtensorMap tm_kv_own,
                 const CUtensorMap* __restrict__ kvmaps, df_comm_t comm, SegInfo segs, __half* __restrict__ out, int lq,
                 int lseg, int heads, int d, int64_t o_pitch, int nseg, int own_seg, int idx, int wait_flags,
                 float scale_log2, Sched sched, float* part_o, float2* part_ml, unsigned int* part_cnt, unsigned int* sched_ctr) {
   constexpr int KSTAGES = Cfg<NBLK>::KST, VSTAGES = Cfg<NBLK>::VST;
-  constexpr uint32_t TMEM_COLS = Cfg<NBLK>::TMEM, TILE_BYTES = NBLK * BLK_BYTES;
+  constexpr uint32_t TILE_BYTES = NBLK * BLK_BYTES;
+  constexpr int SN = Cfg<NBLK>::SN, NSUB = BN / SN;
   using Smem = SmemT<NBLK, KSTAGES, VSTAGES>;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   Smem& sm = *reinterpret_cast<Smem*>(smem_raw);
@@ -139,18 +103,17 @@ fmha_fwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
   // the left-over units are simply whole units of the last round.  With P > 1 (grids that leave most SMs idle: short per-rank Q
   // at n >= 4 with long K/V) a unit's K/V range is cut into P parts that run on otherwise idle SMs; the parts leave
   // un-normalised fp32 partials in the workspace and the LAST part to finish (a ticket per unit) merges them and writes the rows
-  // -- no second kernel.  The roles keep their rings /
-  // barrier phases running across items (tile counter g): TMEM allocation, barrier set-up, tensor-map fetch and pipeline fill
-  // are paid once per CTA, and the K/V loads of the next item run under the epilogue of the current one.
+  // -- no second kernel.  The roles keep their rings / barrier phases running across items (tile counter g): barrier set-up,
+  // tensor-map fetch and pipeline fill are paid once per CTA, and the K/V loads of the next item run under the epilogue of the
+  // current one.
   const int nqt = (lq + BM - 1) / BM;
   const int tps = (lseg + BN - 1) / BN;  // tiles per segment
   const int T_all = nseg * tps;
   const int n_items = sched.a + ((int)blockIdx.x < sched.R * sched.P ? 1 : 0);     // static schedule only
   // item code (from the ring, see the scheduler in the TMA lane) -> Q tile origin, head, batch, first K/V tile, tile count,
   // partial slot (-1: whole unit), left-over index.  Dynamic schedule: the code is the unit; static: the index into this
-  // CTA's list (`a` whole units, then at most one part of a left-over unit).  ITEM_EXACT marks a replay.
-  auto decode = [&](int code, int& q0, int& head, int& bat, int& j_begin, int& T, int& slot, int& lo) {
-    const int it = code & ITEM_MASK;
+  // CTA's list (`a` whole units, then at most one part of a left-over unit).
+  auto decode = [&](int it, int& q0, int& head, int& bat, int& j_begin, int& T, int& slot, int& lo) {
     int u;
     if (sched.dyn) {
       u = it; j_begin = 0; T = T_all; slot = -1; lo = -1;
@@ -169,90 +132,49 @@ fmha_fwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
     bat = rest / heads;
     q0 = qt * BM;
   };
-  // consumer side of the item ring (MMA lane, softmax warps): code of the ui-th item of this CTA, ITEM_END after the last
-  auto fetch = [&](uint32_t ui) -> int {
-    mbar_wait(&sm.sched_full[ui & 1u], (ui >> 1) & 1u);
-    return *(volatile int*)&sm.sched_code[ui & 1u];
-  };
 
-  if (warp == WARP_MMA && lane == 0) {
+  if (threadIdx.x == 0) {
     mbar_init(&sm.q_full, 1);
-    mbar_init(&sm.q_empty, 1);
-    mbar_init(&sm.o_free, NSOFTMAX_WARPS);
-    for (int s = 0; s < KSTAGES; ++s) { mbar_init(&sm.k_full[s], 1); mbar_init(&sm.k_empty[s], 1); }
-    for (int s = 0; s < VSTAGES; ++s) { mbar_init(&sm.v_full[s], 1); mbar_init(&sm.v_empty[s], 1); }
-    mbar_init(&sm.s_full, 1);
-    mbar_init(&sm.s_free, NSOFTMAX_WARPS);
-    mbar_init(&sm.p_full, NSOFTMAX_WARPS);
-    mbar_init(&sm.pv_done, 1);
+    mbar_init(&sm.q_empty, NCONSUMER_WARPS);
+    for (int s = 0; s < KSTAGES; ++s) { mbar_init(&sm.k_full[s], 1); mbar_init(&sm.k_empty[s], NCONSUMER_WARPS); }
+    for (int s = 0; s < VSTAGES; ++s) { mbar_init(&sm.v_full[s], 1); mbar_init(&sm.v_empty[s], NCONSUMER_WARPS); }
     mbar_init(&sm.sched_full[0], 1);
     mbar_init(&sm.sched_full[1], 1);
-    sm.replay_wr = 0; sm.items_done = 0;
-    sm.poison[0] = sm.poison[1] = sm.poison[2] = sm.poison[3] = 0;
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == WARP_TMA) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&sm.tmem_base)), "r"(TMEM_COLS) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = sm.tmem_base;
   pdl_wait();                                          // everything above overlapped the tail of the previous kernel
 
-  if (warp >= NSOFTMAX_WARPS) {
-  if (DF_FMHA_SETMAXNREG && Cfg<NBLK>::CTAS == 2) asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(REGS_PRODUCER));
   if (warp == WARP_TMA) {
-    // =============================================================== TMA producer
+    // =============================================================== scheduler + TMA producer
     if (lane == 0) {
       prefetch_tmap(&tm_q);
       prefetch_tmap(&tm_kv_own);
       uint32_t rd = 0;
       if (nseg > 1) rd = comm.clock[1];
-      // ---- SCHEDULER.  This lane decides what the CTA works on next and tells the other roles through a two-entry ring
-      // (sched_code / sched_full).  Grids that fill the SMs draw whole units from an atomic ticket counter: a CTA that starts
-      // late -- its SM slot was held by a publication kernel of the communication stream -- or runs slower simply takes
-      // fewer units, where the static list made the whole grid wait for it (profiles/r2_exposed_comm_n8.txt).  Small grids
-      // keep their static one-item list (a part of a split unit).  Items that the softmax warps had to abandon (fp32
-      // overflow of the speculative exponent reference, see below) come back through replay_code and are re-run with the
-      // row maxima first; the lane only ends the CTA once every published item has a verdict.
+      // This lane decides what the CTA works on next and tells the consumers through a two-entry ring (sched_code /
+      // sched_full).  Grids that fill the SMs draw whole units from an atomic ticket counter: a CTA that starts late -- its SM
+      // slot was held by a publication kernel of the communication stream -- or runs slower simply takes fewer units.  Small
+      // grids keep their static one-item list (a part of a split unit).  The raw ticket of the next item is drawn one item
+      // ahead: the atomic's latency hides under this item's loads.
       int it_static = 0;
-      // raw ticket of the next fresh item, drawn one item ahead: the atomic's latency hides under this item's loads (the
-      // value is only looked at when the item is scheduled)
       auto draw = [&]() -> unsigned int {
         if (sched.dyn) return atomicAdd(sched_ctr, 1u);
         return (unsigned int)it_static++;
       };
       const unsigned int n_fresh = sched.dyn ? (unsigned int)sched.units : (unsigned int)n_items;
       unsigned int next_t = draw();
-      bool fresh_left = true;
-      uint32_t replay_rd = 0;
-      uint32_t g = 0, ui = 0;                              // K/V tiles and work items issued so far by this CTA
-      for (;; ++ui) {
-        int code;
-        for (;;) {
-          if (replay_rd != sig_load(&sm.replay_wr)) {
-            __threadfence_block();
-            code = (int)sig_load(&sm.replay_code[replay_rd & 7u]) | ITEM_EXACT;
-            ++replay_rd;
-            break;
-          }
-          if (fresh_left) {
-            if (next_t < n_fresh) { code = (int)next_t; next_t = draw(); break; }
-            fresh_left = false;                            // this CTA's one failing draw
-            if (sched.dyn && next_t == n_fresh + gridDim.x - 1u) *sched_ctr = 0u;   // last draw of the launch: self-resetting
-          }
-          if (sig_load(&sm.items_done) == ui) {            // every published item has its verdict ...
-            __threadfence_block();
-            if (replay_rd != sig_load(&sm.replay_wr)) continue;   // ... and the last one asked for a replay
-            code = ITEM_END;
-            break;
-          }
-          __nanosleep(200);
+      uint32_t g = 0;                                      // K/V tiles issued so far by this CTA
+      for (uint32_t ui = 0;; ++ui) {
+        int code = ITEM_END;
+        if (next_t < n_fresh) {
+          code = (int)next_t;
+          next_t = draw();
+        } else if (sched.dyn && next_t == n_fresh + gridDim.x - 1u) {
+          *sched_ctr = 0u;                                 // every CTA fails exactly one draw; the last one resets the counter
         }
         mbar_wait(&sm.q_empty, (ui & 1u) ^ 1u);            // every Q K^T of the previous item has completed: its ring
-        *(volatile int*)&sm.sched_code[ui & 1u] = code;    // entry (item ui - 2's slot) has been read by every role
+        *(volatile int*)&sm.sched_code[ui & 1u] = code;    // entry (item ui - 2's slot) has been read by every consumer
         mbar_arrive(&sm.sched_full[ui & 1u]);
         if (code == ITEM_END) break;
         int q0, head, bat, j_begin, T, slot, lo;
@@ -287,373 +209,194 @@ fmha_fwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
         }
       }
     }
-  } else if (warp == WARP_MMA) {
-    // =============================================================== MMA issuer (single thread)
-    if (lane == 0) {
-      const uint32_t q_addr = smem_u32(sm.q);
-      auto issue_qk = [&](uint32_t g) {
-        const uint32_t st = g % KSTAGES;
-        mbar_wait(&sm.k_full[st], (g / KSTAGES) & 1u);
-        tc_fence_after();
-        const uint32_t k_addr = smem_u32(sm.k[st]);
+  } else {
+    // =============================================================== consumers (warps 0-7): S, softmax, P V, epilogue
+    // Warpgroup wg owns Q rows [64 wg, 64 wg + 64).  In the wgmma accumulator fragment thread t of warp w holds rows
+    // rA = 64 wg + 16 (w & 3) + t/4 and rB = rA + 8, columns 8i + 2(t%4) + {0,1}: s[4i + {0,1}] (row rA), s[4i + {2,3}] (row rB).
+    const int wg = warp >> 2;
+    const int c4 = lane & 3;
+    const int rowA = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+    const uint32_t q_base = smem_u32(sm.q) + wg * 64 * 128;
+    uint32_t g = 0;                                                // K/V tiles processed so far by this CTA (barrier phases)
+    for (uint32_t ui = 0;; ++ui) {
+      mbar_wait(&sm.sched_full[ui & 1u], (ui >> 1) & 1u);
+      const int code = *(volatile int*)&sm.sched_code[ui & 1u];
+      if (code == ITEM_END) break;
+      int q0, head, bat, j_begin, T, slot, lo;
+      decode(code, q0, head, bat, j_begin, T, slot, lo);
+      // exponent references of rows rA / rB, kept NEGATED and in log2 units: P = 2^(S * scale_log2 + n)
+      float nA = INFINITY, nB = INFINITY;
+      float lA = 0.f, lB = 0.f;                                    // partial row sums over this thread's columns
+      float o[NBLK * 32];
 #pragma unroll
-        for (int blk = 0; blk < NBLK; ++blk)
+      for (int i = 0; i < NBLK * 32; ++i) o[i] = 0.f;
+      mbar_wait(&sm.q_full, ui & 1u);
+      int t = j_begin % tps;
+      for (int j = 0; j < T; ++j, ++t, ++g) {
+        if (t == tps) t = 0;
+        const int valid = min(BN, lseg - t * BN);
+        const uint32_t ks = g % KSTAGES, vs = g % VSTAGES;
+        // The tile is processed in NSUB column slices of SN K/V rows (online softmax per slice): for the wider heads two slices of
+        // 64 keep the S fragment at 32 registers next to the larger O fragment.
 #pragma unroll
-          for (int kk = 0; kk < HB / 16; ++kk)
-            mma_ss(tmem + COL_S, smem_desc(q_addr + blk * BLK_BYTES + kk * 32, 16, 1024),
-                   smem_desc(k_addr + blk * BLK_BYTES + kk * 32, 16, 1024), IDESC_S, (blk | kk) > 0);
-        tc_commit(&sm.k_empty[st]);
-        tc_commit(&sm.s_full);
-      };
-      uint32_t g = 0, ui = 0;                              // K/V tiles and work items consumed so far by this CTA
-      for (;; ++ui) {
-        const int code = fetch(ui);
-        if (code == ITEM_END) break;
-        int q0, head, bat, j_begin, T, slot, lo;
-        decode(code, q0, head, bat, j_begin, T, slot, lo);
-        mbar_wait(&sm.q_full, ui & 1u);
-        if (g > 0) {                                       // S still holds the last tile of the previous unit until the
-          mbar_wait(&sm.s_free, (g - 1) & 1u);             // softmax warps have pulled it into registers
-          tc_fence_after();
-        }
-        issue_qk(g);
-        if (T == 1) tc_commit(&sm.q_empty);
-        for (int j = 0; j < T; ++j, ++g) {
-          if (j + 1 < T) {
-            mbar_wait(&sm.s_free, g & 1u);                 // S_j is in the softmax warps' registers
-            tc_fence_after();
-            DF_TR(8, g);
-            issue_qk(g + 1);
-            if (j + 2 == T) tc_commit(&sm.q_empty);        // last Q K^T of this unit: the Q tile may be overwritten once it completes
-            DF_TR(9, g);
-          }
-          const uint32_t st = g % VSTAGES;
-          mbar_wait(&sm.p_full, g & 1u);
-          mbar_wait(&sm.v_full[st], (g / VSTAGES) & 1u);
-          if (j == 0 && ui > 0) mbar_wait(&sm.o_free, (ui - 1) & 1u);   // previous unit's O has left TMEM
-          tc_fence_after();
-          DF_TR(10, g);
-          const uint32_t v_addr = smem_u32(sm.v[st]);
+        for (int sub = 0; sub < NSUB; ++sub) {
+          // ---- S = Q K_j^T (this slice)
+          float s[SN / 2];
+          if (sub == 0) mbar_wait(&sm.k_full[ks], (g / KSTAGES) & 1u);
+          const uint32_t k_addr = smem_u32(sm.k[ks]) + sub * SN * 128;
+          wgmma_fence();
 #pragma unroll
           for (int blk = 0; blk < NBLK; ++blk)
 #pragma unroll
-            for (int kk = 0; kk < BN / 16; ++kk)
-              mma_ts(tmem + COL_O + blk * HB, tmem + COL_P + kk * 8, smem_desc(v_addr + blk * BLK_BYTES + kk * 2048, 16384, 1024),
-                     IDESC_PV, (j > 0 || kk > 0) ? 1u : 0u);
-          tc_commit(&sm.v_empty[st]);
-          tc_commit(&sm.pv_done);
-          DF_TR(11, g);
-        }
-      }
-    }
-  }
-  } else {
-    if (DF_FMHA_SETMAXNREG && Cfg<NBLK>::CTAS == 2) asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(REGS_SOFTMAX));
-    // =============================================================== softmax / correction / epilogue (warps 0-7)
-    // Warp w owns 16 rows (TMEM lanes 32*(w&3) + 16*(w>>2) ..+15) and ALL 128 S columns of them, in the 16x256b fragment
-    // layout: thread t holds rows rA = t/4 and rB = t/4 + 8, columns 8i + 2(t%4) + {0,1} for i = 0..15 (64 values).  A row
-    // lives in one quad, so the row maximum is two shuffles -- no shared-memory exchange and no named barrier between warps
-    // (v2 split rows over two warps and paid an STS + 64-thread bar.sync + LDS per tile).  A software-pipelined variant (v4:
-    // 64-column sub-tiles, the next sub-tile's tcgen05.ld under the current exponentials) measured 25 % SLOWER -- the kernel is
-    // bound by issue slots + dependency stalls at the 96-register cap, not by the TMEM-load latency it hid
-    // (profiles/r2_attn_sweep_v4.txt) -- and was removed.
-    const int quad = warp & 3, hr = warp >> 2;
-    const uint32_t lane16 = (uint32_t)(quad * 32 + hr * 16);
-    uint32_t lane_base = tmem + (lane16 << 16);
-    // shared-window address of the barrier block, computed once: left to itself ptxas rebuilds it (S2R SR_CgaCtaId + LEA)
-    // and lane_base (S2R SR_TID + 5 ALU ops) at every use inside the tile loop instead of holding two registers
-    uint32_t bars = smem_u32(&sm.q_full);
-#if DF_OPAQUE_BASES
-    asm volatile("" : "+r"(lane_base), "+r"(bars));
-#endif
-#define DF_BAR(member) (bars + (uint32_t)(offsetof(Smem, member) - offsetof(Smem, q_full)))
-    const int c4 = lane & 3, r8 = lane >> 2;
-    constexpr bool SPECULATE = Cfg<NBLK>::CTAS == 2;               // see "speculative exponent reference" below
-    uint32_t g = 0, ui = 0;                                        // K/V tiles / work items processed so far by this CTA (barrier phases)
-    for (;; ++ui) {
-    const int code = fetch(ui);
-    if (code == ITEM_END) break;
-    int q0, head, bat, j_begin, T, slot, lo;
-    decode(code, q0, head, bat, j_begin, T, slot, lo);
-    // exponent references of rows rA / rB, kept NEGATED and in log2 units: P = 2^(S * scale_log2 + n)
-    float nA = INFINITY, nB = INFINITY;
-    float lA = 0.f, lB = 0.f;                                      // partial row sums over this thread's columns
-    int t = j_begin % tps;
-    for (int j = 0; j < T; ++j, ++t, ++g) {
-      if (t == tps) t = 0;
-      const int valid = min(BN, lseg - t * BN);
-      mbar_wait(DF_BAR(s_full), g & 1u);
-      tc_fence_after();
-      if (threadIdx.x == 0) DF_TR(0, g);
-      uint32_t sr[64];
-      tmem_ld_16x256b_x8(lane_base + COL_S, sr);        // two x8 loads (one x16 exceeds what ptxas accepts under the 80-register
-      tmem_ld_16x256b_x8(lane_base + COL_S + 64, sr + 32);   // launch bound, whatever setmaxnreg grants later), one wait
-      tmem_wait_ld();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(DF_BAR(s_free));      // the tensor core may overwrite S with Q K_{j+1}^T now
-      if (threadIdx.x == 0) DF_TR(1, g);
-      if (valid < BN) {                                // ragged last tile of a segment only (warp-uniform branch)
-        asm volatile("" ::: "memory");
-#pragma unroll
-        for (int i = 0; i < 16; ++i)
-#pragma unroll
-          for (int k = 0; k < 2; ++k)
-            if (8 * i + 2 * c4 + k >= valid) { sr[4 * i + k] = 0xff800000u; sr[4 * i + 2 + k] = 0xff800000u; }
-      }
-      // SPECULATIVE EXPONENT REFERENCE (two-CTAs-per-SM configuration).  Only the first tile of an item computes the row maxima
-      // before its exponentials.  Every later tile exponentiates against the reference it inherited -- no FMNMX pass, no quad
-      // shuffles, no max -> exp dependency -- and then proves the guess was harmless: P is stored as fp16, so it is enough
-      // that no value reached 2^13, which the row sums the tile needs anyway show (a thread's 32 values of a row sum to more
-      // than 2^13 only if one of them exceeded 2^8; the polynomial lanes, whose exponent insertion wraps for x >= 128, are
-      // covered by the largest integer part they produced).  S has long been released by then; a failing tile is repaired
-      // IN REGISTERS: the exponentials are still exact fp32 values, so their row maxima give the new reference as a power
-      // of two and P, l, O are rescaled by it -- no second look at S.  Only when an exponential overflowed fp32 itself (a logit
-      // 88 nats above the reference) is the information gone: the warp marks the item poisoned, the CTA finishes it without
-      // publishing anything and the scheduler re-runs it with the maxima first (ITEM_EXACT).
-      const bool exact = !SPECULATE || (code & ITEM_EXACT) != 0 || j == 0;
-      // O of this warp's 16 rows *= alpha (rare: the reference moved).  Called warp-uniformly; waits for P V_{j-1} first --
-      // the regular wait further down then finds the phase complete.  Keeping this out of the common path also keeps
-      // alpha / moved out of its live registers (the loop runs at the 96-register cap of two CTAs per SM).
-      auto rescale_o = [&](float alphaA, float alphaB) {
-        if (j == 0) return;
-        mbar_wait(DF_BAR(pv_done), (g - 1) & 1u);
-        tc_fence_after();
-#pragma unroll 1
-        for (int c = 0; c < NBLK * HB; c += 16) {      // 16 columns (8 registers) at a time: S is live around this call
-          uint32_t o[8];
-          tmem_ld_16x256b_x2(lane_base + COL_O + c, o);
-          tmem_wait_ld();
-          o[0] = __float_as_uint(__uint_as_float(o[0]) * alphaA); o[1] = __float_as_uint(__uint_as_float(o[1]) * alphaA);
-          o[2] = __float_as_uint(__uint_as_float(o[2]) * alphaB); o[3] = __float_as_uint(__uint_as_float(o[3]) * alphaB);
-          o[4] = __float_as_uint(__uint_as_float(o[4]) * alphaA); o[5] = __float_as_uint(__uint_as_float(o[5]) * alphaA);
-          o[6] = __float_as_uint(__uint_as_float(o[6]) * alphaB); o[7] = __float_as_uint(__uint_as_float(o[7]) * alphaB);
-          tmem_st_16x256b_x2(lane_base + COL_O + c, o);
-        }
-        tmem_wait_st();
-      };
-      if (exact) {
-        float mA0 = -INFINITY, mA1 = -INFINITY, mB0 = -INFINITY, mB1 = -INFINITY;   // two chains per row
-#pragma unroll
-        for (int i = 0; i < 16; i += 2) {
-          mA0 = max3(mA0, __uint_as_float(sr[4 * i]), __uint_as_float(sr[4 * i + 1]));
-          mB0 = max3(mB0, __uint_as_float(sr[4 * i + 2]), __uint_as_float(sr[4 * i + 3]));
-          mA1 = max3(mA1, __uint_as_float(sr[4 * i + 4]), __uint_as_float(sr[4 * i + 5]));
-          mB1 = max3(mB1, __uint_as_float(sr[4 * i + 6]), __uint_as_float(sr[4 * i + 7]));
-        }
-        float mA = fmaxf(mA0, mA1), mB = fmaxf(mB0, mB1);
-        mA = fmaxf(mA, __shfl_xor_sync(0xffffffffu, mA, 1));
-        mB = fmaxf(mB, __shfl_xor_sync(0xffffffffu, mB, 1));
-        mA = fmaxf(mA, __shfl_xor_sync(0xffffffffu, mA, 2));
-        mB = fmaxf(mB, __shfl_xor_sync(0xffffffffu, mB, 2));
-        if (threadIdx.x == 0) DF_TR(2, g);
-        // lazy rescale: keep the old reference while the max moved by < 2^8
-        const float dA = fmaf(mA, scale_log2, nA), dB = fmaf(mB, scale_log2, nB);      // log2 of the largest P of the tile
-        float alphaA = 1.f, alphaB = 1.f;
-        if (dA > 8.f) { alphaA = ex2(-dA); nA = -mA * scale_log2; lA *= alphaA; }
-        if (dB > 8.f) { alphaB = ex2(-dB); nB = -mB * scale_log2; lB *= alphaB; }
-        if (__any_sync(0xffffffffu, dA > 8.f || dB > 8.f)) rescale_o(alphaA, alphaB);
-      }
-      const uint64_t scale2 = pack2(scale_log2, scale_log2), nA2 = pack2(nA, nA), nB2 = pack2(nB, nB);
-      uint64_t sA = pack2(0.f, 0.f), sB = pack2(0.f, 0.f);
-      float tmax = 0.f;                                // largest (1.5 * 2^23 + integer part) of the polynomial lanes
-#pragma unroll
-      for (int i = 0; i < 16; ++i) {                   // exponentials IN PLACE (fp32): nothing leaves the registers before the check
-        const uint64_t xA = fma2(pack2(__uint_as_float(sr[4 * i]), __uint_as_float(sr[4 * i + 1])), scale2, nA2);
-        const uint64_t xB = fma2(pack2(__uint_as_float(sr[4 * i + 2]), __uint_as_float(sr[4 * i + 3])), scale2, nB2);
-        float a0, a1, b0, b1;
-        if ((i * DF_EMU_GROUPS) / 16 != ((i + 1) * DF_EMU_GROUPS) / 16) {             // this share of the exponentials runs on the FMA / ALU pipes
-          ex2_poly2(xA, a0, a1, tmax);
-          ex2_poly2(xB, b0, b1, tmax);
-        } else {
-          float x0, x1;
-          unpack2(xA, x0, x1); a0 = ex2(x0); a1 = ex2(x1);
-          unpack2(xB, x0, x1); b0 = ex2(x0); b1 = ex2(x1);
-        }
-        sA = add2(sA, pack2(a0, a1));
-        sB = add2(sB, pack2(b0, b1));
-        sr[4 * i] = __float_as_uint(a0); sr[4 * i + 1] = __float_as_uint(a1);
-        sr[4 * i + 2] = __float_as_uint(b0); sr[4 * i + 3] = __float_as_uint(b1);
-      }
-      float tA, tB;
-      {
-        float s0, s1;
-        unpack2(sA, s0, s1); tA = s0 + s1;
-        unpack2(sB, s0, s1); tB = s0 + s1;
-      }
-      if (!exact) {
-        const bool over = !(tA <= 8192.f) || !(tB <= 8192.f) || tmax > 12582912.f + 13.f;   // also true for NaN sums
-        if (__any_sync(0xffffffffu, over)) {           // rare: the inherited reference was too small for this tile
-          const bool lost = !(tA < 3.0e38f) || !(tB < 3.0e38f) || tmax > 12582912.f + 126.f;
-          if (__any_sync(0xffffffffu, lost)) {           // fp32 overflow: only S could tell the values apart, and S is gone
-            if (lane == 0) *(volatile int*)&sm.poison[ui & 3u] = 1;
-          } else {
-            float pA = 0.f, pB = 0.f;
-#pragma unroll
-            for (int i = 0; i < 16; ++i) {
-              pA = max3(pA, __uint_as_float(sr[4 * i]), __uint_as_float(sr[4 * i + 1]));
-              pB = max3(pB, __uint_as_float(sr[4 * i + 2]), __uint_as_float(sr[4 * i + 3]));
+            for (int kk = 0; kk < HB / 16; ++kk)
+              wgmma_ss<SN>(s, smem_desc(q_base + blk * BLK_BYTES + kk * 32, 16, 1024), smem_desc(k_addr + blk * BLK_BYTES + kk * 32, 16, 1024),
+                           (blk | kk) > 0);
+          wgmma_commit();
+          wgmma_wait<0>();
+          fence_regs<SN / 2>(s);
+          if (sub == NSUB - 1) {
+            __syncwarp();
+            if (lane == 0) {
+              mbar_arrive(&sm.k_empty[ks]);
+              if (j + 1 == T) mbar_arrive(&sm.q_empty);    // last Q K^T of this item: the Q tile may be overwritten
             }
-            pA = fmaxf(pA, __shfl_xor_sync(0xffffffffu, pA, 1)); pB = fmaxf(pB, __shfl_xor_sync(0xffffffffu, pB, 1));
-            pA = fmaxf(pA, __shfl_xor_sync(0xffffffffu, pA, 2)); pB = fmaxf(pB, __shfl_xor_sync(0xffffffffu, pB, 2));
-            // shift the reference by the exponent of the row maximum (rows that stayed below 2 keep theirs): exact powers of two
-            const int kA = max(0, (int)((__float_as_uint(pA) >> 23) & 0xffu) - 127), kB = max(0, (int)((__float_as_uint(pB) >> 23) & 0xffu) - 127);
-            const float alphaA = __uint_as_float((uint32_t)(127 - kA) << 23), alphaB = __uint_as_float((uint32_t)(127 - kB) << 23);
-            nA -= (float)kA; nB -= (float)kB;
-            lA *= alphaA; lB *= alphaB; tA *= alphaA; tB *= alphaB;
-#pragma unroll
-            for (int i = 0; i < 16; ++i) {
-              sr[4 * i] = __float_as_uint(__uint_as_float(sr[4 * i]) * alphaA);
-              sr[4 * i + 1] = __float_as_uint(__uint_as_float(sr[4 * i + 1]) * alphaA);
-              sr[4 * i + 2] = __float_as_uint(__uint_as_float(sr[4 * i + 2]) * alphaB);
-              sr[4 * i + 3] = __float_as_uint(__uint_as_float(sr[4 * i + 3]) * alphaB);
-            }
-            rescale_o(alphaA, alphaB);
           }
+          const int vcols = valid - sub * SN;              // valid columns of this slice
+          if (vcols < SN) {                                // ragged last tile of a segment only (warp-uniform branch)
+#pragma unroll
+            for (int i = 0; i < SN / 8; ++i)
+#pragma unroll
+              for (int k = 0; k < 2; ++k)
+                if (8 * i + 2 * c4 + k >= vcols) { s[4 * i + k] = -INFINITY; s[4 * i + 2 + k] = -INFINITY; }
+          }
+          // ---- row maxima; lazy rescale: keep the old reference while the maximum moved by < 2^8 (P stays below 2^8 in fp16)
+          float mA0 = -INFINITY, mA1 = -INFINITY, mB0 = -INFINITY, mB1 = -INFINITY;   // two chains per row
+#pragma unroll
+          for (int i = 0; i < SN / 8; i += 2) {
+            mA0 = fmaxf(mA0, fmaxf(s[4 * i], s[4 * i + 1]));
+            mB0 = fmaxf(mB0, fmaxf(s[4 * i + 2], s[4 * i + 3]));
+            mA1 = fmaxf(mA1, fmaxf(s[4 * i + 4], s[4 * i + 5]));
+            mB1 = fmaxf(mB1, fmaxf(s[4 * i + 6], s[4 * i + 7]));
+          }
+          float mA = fmaxf(mA0, mA1), mB = fmaxf(mB0, mB1);
+          mA = fmaxf(mA, __shfl_xor_sync(0xffffffffu, mA, 1));
+          mB = fmaxf(mB, __shfl_xor_sync(0xffffffffu, mB, 1));
+          mA = fmaxf(mA, __shfl_xor_sync(0xffffffffu, mA, 2));
+          mB = fmaxf(mB, __shfl_xor_sync(0xffffffffu, mB, 2));
+          const float dA = fmaf(mA, scale_log2, nA), dB = fmaf(mB, scale_log2, nB);    // log2 of the largest P of the slice
+          if (dA > 8.f) {
+            const float alpha = ex2(-dA);
+            nA = -mA * scale_log2; lA *= alpha;
+#pragma unroll
+            for (int i = 0; i < NBLK * 8; ++i) { o[4 * i] *= alpha; o[4 * i + 1] *= alpha; }
+          }
+          if (dB > 8.f) {
+            const float alpha = ex2(-dB);
+            nB = -mB * scale_log2; lB *= alpha;
+#pragma unroll
+            for (int i = 0; i < NBLK * 8; ++i) { o[4 * i + 2] *= alpha; o[4 * i + 3] *= alpha; }
+          }
+          // ---- P = 2^(S * scale_log2 + n), row sums, packed to fp16 as the A fragment of the P V wgmmas
+          uint32_t pk[SN / 4];
+#pragma unroll
+          for (int i = 0; i < SN / 8; ++i) {
+            const int grp = sub * (SN / 8) + i;            // column group of the 128-wide tile row
+            float e[4];
+#pragma unroll
+            for (int k = 0; k < 4; ++k) {
+              const float x = fmaf(s[4 * i + k], scale_log2, k < 2 ? nA : nB);
+              e[k] = ((grp * DF_EMU_GROUPS) / 16 != ((grp + 1) * DF_EMU_GROUPS) / 16) ? ex2_poly(x) : ex2(x);
+            }
+            lA += e[0] + e[1];
+            lB += e[2] + e[3];
+            pk[2 * i] = pack_h2(e[0], e[1]);
+            pk[2 * i + 1] = pack_h2(e[2], e[3]);
+          }
+          // ---- O += P V_j (this slice's K/V rows)
+          if (sub == 0) mbar_wait(&sm.v_full[vs], (g / VSTAGES) & 1u);
+          const uint32_t v_addr = smem_u32(sm.v[vs]) + sub * SN * 128;
+          wgmma_fence();
+#pragma unroll
+          for (int kk = 0; kk < SN / 16; ++kk)
+#pragma unroll
+            for (int blk = 0; blk < NBLK; ++blk)
+              wgmma_rs_n64(o + 32 * blk, pk + 4 * kk, smem_desc(v_addr + blk * BLK_BYTES + kk * 2048, 16384, 1024), 1u);
+          wgmma_commit();
+          wgmma_wait<0>();
+          fence_regs<NBLK * 32>(o);
         }
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&sm.v_empty[vs]);
       }
-      lA += tA;
-      lB += tB;
-      if (threadIdx.x == 0) DF_TR(3, g);
-      // P -> fp16 -> TMEM in two halves of 32 packed columns (16 instead of 32 packed registers live at a time)
+      // ---- epilogue: quad-reduce the row sums, then O / l -> fp16 -> HBM (or an fp32 partial of a split unit)
+      lA += __shfl_xor_sync(0xffffffffu, lA, 1); lB += __shfl_xor_sync(0xffffffffu, lB, 1);
+      lA += __shfl_xor_sync(0xffffffffu, lA, 2); lB += __shfl_xor_sync(0xffffffffu, lB, 2);
+      const bool partial = slot >= 0;
+      bool finish = !partial;                            // this CTA writes the output rows
+      float denA = lA, denB = lB;
+      if (partial) {
+        // ---- un-normalised fp32 partial (reference -n) -> workspace; the last part of this unit to arrive merges
+        const int64_t prow = (int64_t)slot * BM + rowA;                  // row of this part's partial in the workspace
+        if (c4 == 0) { part_ml[prow] = make_float2(-nA, lA); part_ml[prow + 8] = make_float2(-nB, lB); }
 #pragma unroll
-      for (int hf = 0; hf < 2; ++hf) {
-        uint32_t pr[16];
-#pragma unroll
-        for (int ii = 0; ii < 8; ++ii) {
-          const int i = hf * 8 + ii;
-          pr[2 * ii] = pack_h2(__uint_as_float(sr[4 * i]), __uint_as_float(sr[4 * i + 1]));
-          pr[2 * ii + 1] = pack_h2(__uint_as_float(sr[4 * i + 2]), __uint_as_float(sr[4 * i + 3]));
+        for (int i = 0; i < NBLK * 8; ++i) {
+          const int col = 8 * i + 2 * c4;
+          *reinterpret_cast<float2*>(part_o + prow * (NBLK * HB) + col) = make_float2(o[4 * i], o[4 * i + 1]);
+          *reinterpret_cast<float2*>(part_o + (prow + 8) * (NBLK * HB) + col) = make_float2(o[4 * i + 2], o[4 * i + 3]);
         }
-        if (hf == 0 && j > 0) {
-          mbar_wait(DF_BAR(pv_done), (g - 1) & 1u);  // P buffer free, O quiescent
-          tc_fence_after();
-          if (threadIdx.x == 0) DF_TR(4, g);
-        }
-        tmem_st_16x128b_x8(lane_base + COL_P + hf * 32, pr);
-      }
-      tmem_wait_st();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(DF_BAR(p_full));
-      if (threadIdx.x == 0) DF_TR(5, g);
-    }
-    // ---- epilogue: row sums / references -> shared memory (quad reduce), then O / l -> fp16 -> HBM in the 32x32b layout
-    //      (thread = row, 16-byte stores): warp w writes columns [32*(w>>2), +32) of the 32 rows of its lane quarter
-    lA += __shfl_xor_sync(0xffffffffu, lA, 1); lB += __shfl_xor_sync(0xffffffffu, lB, 1);
-    lA += __shfl_xor_sync(0xffffffffu, lA, 2); lB += __shfl_xor_sync(0xffffffffu, lB, 2);
-    if (c4 == 0) {
-      sm.red_sum[ui & 1][lane16 + r8] = lA; sm.red_sum[ui & 1][lane16 + r8 + 8] = lB;
-      sm.red_ref[ui & 1][lane16 + r8] = -nA; sm.red_ref[ui & 1][lane16 + r8 + 8] = -nB;
-    }
-    asm volatile("bar.sync 1, 256;" ::: "memory");
-    const bool item_bad = SPECULATE && *(volatile int*)&sm.poison[ui & 3u] != 0;
-    if (threadIdx.x == 0) {                           // verdict for the scheduler: replay request, then the done counter
-      sm.poison[(ui + 2u) & 3u] = 0;                  // the entry two items ahead (nobody reads or sets it now)
-      if (item_bad) {
-        const uint32_t wr = sig_load(&sm.replay_wr);  // this thread is the only writer
-        sig_store(&sm.replay_code[wr & 7u], (uint32_t)(code & ITEM_MASK));
-        __threadfence_block();
-        sig_store(&sm.replay_wr, wr + 1u);
-      }
-      __threadfence_block();
-      sig_store(&sm.items_done, ui + 1u);
-    }
-    const int half = hr;
-    const int row = quad * 32 + lane;
-    const uint32_t row_base = tmem + ((uint32_t)(quad * 32) << 16);
-    const float l_row = sm.red_sum[ui & 1][row];        // [unit parity]: a fast warp may already be filling the next unit's sums
-    const float m_ref = sm.red_ref[ui & 1][row];
-    mbar_wait(DF_BAR(pv_done), (g - 1) & 1u);
-    tc_fence_after();
-    const bool partial = slot >= 0 && !item_bad;     // a poisoned item publishes nothing: its replay will
-    const int64_t prow = (int64_t)(partial ? slot : 0) * BM + row;          // row of this part's partial in the workspace
-    if (partial && half == 0) part_ml[prow] = make_float2(m_ref, l_row);
-    uint32_t o[NBLK][32];
-#pragma unroll
-    for (int blk = 0; blk < NBLK; ++blk) tmem_ld32(row_base + COL_O + blk * HB + half * 32, o[blk]);
-    tmem_wait_ld();
-    tc_fence_before();                                // O is in registers: the next item's first P V may overwrite the accumulator
-    __syncwarp();
-    if (lane == 0) mbar_arrive(DF_BAR(o_free));
-    bool finish = !partial && !item_bad;              // this CTA writes the output rows
-    float m_all = m_ref, denom = l_row, w_own = 1.f;
-    if (partial) {
-      // ---- un-normalised fp32 partial (reference max m_ref) -> workspace; the last part of this unit to arrive merges
-#pragma unroll
-      for (int blk = 0; blk < NBLK; ++blk) {
-        float* dst = part_o + prow * (NBLK * HB) + blk * HB + half * 32;
-#pragma unroll
-        for (int vq = 0; vq < 8; ++vq)
-          st_v4(dst + vq * 4, make_int4((int)o[blk][vq * 4], (int)o[blk][vq * 4 + 1], (int)o[blk][vq * 4 + 2], (int)o[blk][vq * 4 + 3]));
-      }
-      __threadfence();
-      asm volatile("bar.sync 1, 256;" ::: "memory");
-      if (threadIdx.x == 0) {
-        const unsigned int tk = atomicAdd(part_cnt + lo, 1u);
-        sm.ticket = tk;
-        if (tk == (unsigned int)sched.P - 1) part_cnt[lo] = 0;        // self-resetting: the next launch is stream-ordered
-      }
-      asm volatile("bar.sync 1, 256;" ::: "memory");
-      finish = sm.ticket == (unsigned int)sched.P - 1;
-      if (finish) {
         __threadfence();
-        // merge: out = sum_p w_p O_p / sum_p w_p l_p,  w_p = 2^((m_p - max_p m_p) * scale)   (parts of unit `lo`: slots lo*P ..)
-        const int s0 = lo * sched.P;
-        float m_max = -INFINITY;
-        for (int pp = 0; pp < sched.P; ++pp) m_max = fmaxf(m_max, ld_f2(part_ml + (int64_t)(s0 + pp) * BM + row).x);
-        m_all = m_max;
-        denom = 0.f;
+        asm volatile("bar.sync 1, 256;" ::: "memory");
+        if (threadIdx.x == 0) {
+          const unsigned int tk = atomicAdd(part_cnt + lo, 1u);
+          sm.ticket = tk;
+          if (tk == (unsigned int)sched.P - 1) part_cnt[lo] = 0;        // self-resetting: the next launch is stream-ordered
+        }
+        asm volatile("bar.sync 1, 256;" ::: "memory");
+        finish = sm.ticket == (unsigned int)sched.P - 1;
+        if (finish) {
+          __threadfence();
+          // merge: out = sum_p w_p O_p / sum_p w_p l_p,  w_p = 2^(m_p - max_p m_p)   (parts of unit `lo`: slots lo*P ..)
+          const int s0 = lo * sched.P;
 #pragma unroll
-        for (int blk = 0; blk < NBLK; ++blk)
+          for (int h = 0; h < 2; ++h) {
+            const int64_t r = rowA + 8 * h;
+            float m_max = -INFINITY;
+            for (int pp = 0; pp < sched.P; ++pp) m_max = fmaxf(m_max, ld_f2(part_ml + (int64_t)(s0 + pp) * BM + r).x);
+            float den = 0.f;
 #pragma unroll
-          for (int c = 0; c < 32; ++c) o[blk][c] = 0u;
-        for (int pp = 0; pp < sched.P; ++pp) {
-          const float2 ml = ld_f2(part_ml + (int64_t)(s0 + pp) * BM + row);
-          const float w = ex2(ml.x - m_max);          // references are kept in log2 units
-          denom = fmaf(w, ml.y, denom);
+            for (int i = 0; i < NBLK * 8; ++i) { o[4 * i + 2 * h] = 0.f; o[4 * i + 2 * h + 1] = 0.f; }
+            for (int pp = 0; pp < sched.P; ++pp) {
+              const float2 ml = ld_f2(part_ml + (int64_t)(s0 + pp) * BM + r);
+              const float w = ex2(ml.x - m_max);        // references are kept in log2 units
+              den = fmaf(w, ml.y, den);
+              const float2* src = reinterpret_cast<const float2*>(part_o + ((int64_t)(s0 + pp) * BM + r) * (NBLK * HB));
 #pragma unroll
-          for (int blk = 0; blk < NBLK; ++blk) {
-            const float* src = part_o + ((int64_t)(s0 + pp) * BM + row) * (NBLK * HB) + blk * HB + half * 32;
-#pragma unroll
-            for (int vq = 0; vq < 8; ++vq) {
-              const int4 v = ld_v4(src + vq * 4);
-              o[blk][vq * 4 + 0] = __float_as_uint(fmaf(w, __int_as_float(v.x), __uint_as_float(o[blk][vq * 4 + 0])));
-              o[blk][vq * 4 + 1] = __float_as_uint(fmaf(w, __int_as_float(v.y), __uint_as_float(o[blk][vq * 4 + 1])));
-              o[blk][vq * 4 + 2] = __float_as_uint(fmaf(w, __int_as_float(v.z), __uint_as_float(o[blk][vq * 4 + 2])));
-              o[blk][vq * 4 + 3] = __float_as_uint(fmaf(w, __int_as_float(v.w), __uint_as_float(o[blk][vq * 4 + 3])));
+              for (int i = 0; i < NBLK * 8; ++i) {
+                const float2 v = ld_f2(src + 4 * i + c4);
+                o[4 * i + 2 * h] = fmaf(w, v.x, o[4 * i + 2 * h]);
+                o[4 * i + 2 * h + 1] = fmaf(w, v.y, o[4 * i + 2 * h + 1]);
+              }
             }
+            if (h == 0) denA = den; else denB = den;
           }
         }
       }
-    }
-    (void)m_all; (void)w_own;
-    if (finish && q0 + row < lq) {
-      const float inv = 1.f / denom;
+      if (finish) {
 #pragma unroll
-      for (int blk = 0; blk < NBLK; ++blk) {
-        const int col0 = blk * HB + half * 32;        // first head column of this chunk
-        __half* dst = out + ((int64_t)bat * lq + q0 + row) * o_pitch + (int64_t)head * d + col0;
-        const int nvec = (d - col0) / 8;              // 16-byte vectors of real (un-padded) head columns in this chunk
+        for (int h = 0; h < 2; ++h) {
+          const int row = rowA + 8 * h;
+          if (q0 + row >= lq) continue;
+          const float inv = 1.f / (h == 0 ? denA : denB);
+          __half* dst = out + ((int64_t)bat * lq + q0 + row) * o_pitch + (int64_t)head * d;
 #pragma unroll
-        for (int vq = 0; vq < 4; ++vq) {
-          if (vq < nvec) {
-            int4 w;
-            w.x = pack_h2(__uint_as_float(o[blk][vq * 8 + 0]) * inv, __uint_as_float(o[blk][vq * 8 + 1]) * inv);
-            w.y = pack_h2(__uint_as_float(o[blk][vq * 8 + 2]) * inv, __uint_as_float(o[blk][vq * 8 + 3]) * inv);
-            w.z = pack_h2(__uint_as_float(o[blk][vq * 8 + 4]) * inv, __uint_as_float(o[blk][vq * 8 + 5]) * inv);
-            w.w = pack_h2(__uint_as_float(o[blk][vq * 8 + 6]) * inv, __uint_as_float(o[blk][vq * 8 + 7]) * inv);
-            st_v4(dst + vq * 8, w);
+          for (int i = 0; i < NBLK * 8; ++i) {
+            const int col = 8 * i + 2 * c4;
+            if (col < d)                                 // d % 8 == 0: a column pair is entirely inside or outside the head
+              *reinterpret_cast<uint32_t*>(dst + col) = pack_h2(o[4 * i + 2 * h] * inv, o[4 * i + 2 * h + 1] * inv);
           }
         }
       }
-    }
-    }   // work units
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == WARP_TMA) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(TMEM_COLS) : "memory");
+    }   // work items
   }
 }
 
@@ -719,7 +462,7 @@ int sm_count() {
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    if (sms <= 0) sms = 148;
+    if (sms <= 0) sms = kSmCount;
   }
   return sms;
 }
@@ -727,13 +470,12 @@ int sm_count() {
 #define DF_MIN_PART_TILES 8    // a part of a split unit keeps at least this many K/V tiles (Q load + partial write + merge per part)
 #endif
 // Grid and work schedule of a launch (see the kernel): G resident CTAs, `a` whole units per CTA, R left-over units in P parts.
-// Measured policy (profiles/r2_attn_tail_split.txt): cutting the left-over units of a grid that already fills the SMs does
-// not pay -- the R CTAs of the last round have their SMs to themselves and run ~1.6x faster per tile, which a balanced tail
-// trades for partial writes and a merge (SDXL 1024^2: level 1 144 vs 136 us, level 2 32.5 vs 30.4 us) -- so P > 1 only when the
-// units leave at least half of the CTA slots idle AND every part keeps >= 8 K/V tiles (n = 4 level 1: 41.6 -> 37.7 us).
+// Policy: the left-over units of a grid that already fills the SMs are not cut -- the R CTAs of the last round have the memory
+// system to themselves, which a balanced tail would trade for partial writes and a merge -- so P > 1 only when the units leave
+// at least half of the SMs idle AND every part keeps >= 8 K/V tiles.
 void plan_schedule(int b, int lq, int lseg, int nseg, int heads, int d, bool have_ws, int& grid, Sched& sc) {
-  const int nblk = (d + HB - 1) / HB;
-  const long long slots = (long long)sm_count() * (nblk == 1 ? Cfg<1>::CTAS : 1);
+  (void)d;
+  const long long slots = sm_count();
   const long long units = (long long)((lq + BM - 1) / BM) * heads * b;
   const int t_all = nseg * ((lseg + BN - 1) / BN);
   sc.units = (int)units;
@@ -760,14 +502,6 @@ size_t workspace_need(const Sched& sc, int d) {
   return WS_HEADER + 1024 + ((size_t)sc.R * sizeof(unsigned int) + 255) / 256 * 256 + parts * BM * sizeof(float2) + parts * BM * hd_pad * sizeof(float);
 }
 }  // namespace
-
-#ifdef DF_TRACE
-extern "C" int df_debug_read_trace(long long* out_host /* 64*16 */) {
-  DF_CHECK_CUDA(cudaDeviceSynchronize());
-  DF_CHECK_CUDA(cudaMemcpyFromSymbol(out_host, df_trace_buf, sizeof(long long) * 64 * 16));
-  return 0;
-}
-#endif
 
 extern "C" size_t df_attn_workspace_bytes(int b, int lq, int lseg, int nseg, int heads, int d) {
   int grid;

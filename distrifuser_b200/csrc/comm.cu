@@ -20,7 +20,7 @@ void set_error(const char* fmt, ...) {
 unsigned df::pdl_mask() {
   static int v = -1;
   if (v < 0) {
-    const char* e = getenv("DF_PDL");          // opt-in: measured neutral on a 1-GPU 1024^2 step (profiles/r2_pdl_ab.txt)
+    const char* e = getenv("DF_PDL");          // opt-in (off by default)
     v = e ? atoi(e) : 0;
     if (v < 0) v = 0;
   }
@@ -109,9 +109,8 @@ __device__ __forceinline__ void signal_when_last(const df_comm_t& c, int idx, ui
 }
 
 // 128 threads, DF_PUB_UNROLL 16-byte loads in flight per thread: the transfer is bound by how many loads are outstanding (local
-// read latency ~1 us; the peer stores are posted).  Measured on 2 x B200 (profiles/r2_exposed_comm_n2.txt): 64 CTAs x 2 loads
-// exposed 1.02 ms per asynchronous step, 64 CTAs x 8 loads 0.60 ms (24 CTAs: 0.91, 8 CTAs: 0.73) -- what is exposed is the tail
-// of the step's last publications, so the faster transfer wins over taking fewer SM slots.
+// read latency ~1 us; the peer stores are posted).  What is exposed is the tail of the step's last publications, so a faster
+// transfer wins over taking fewer SM slots.
 #ifndef DF_PUB_UNROLL
 #define DF_PUB_UNROLL 8
 #endif

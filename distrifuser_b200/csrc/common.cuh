@@ -1,4 +1,4 @@
-// distrifuser_b200 -- shared device/host helpers (sm_100a only).
+// distrifuser_b200 -- shared device/host helpers (sm_90a only).
 #pragma once
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
@@ -8,6 +8,9 @@
 #include "../../include/distrifuser_b200.h"
 
 namespace df {
+
+// SMs of the H100 SXM the grid-size heuristics are tuned for (kernels that size a persistent grid query the device)
+constexpr int kSmCount = 132;
 
 void set_error(const char* fmt, ...);
 
@@ -88,7 +91,7 @@ __device__ __forceinline__ void st_v4(void* p, const int4& v) {
 
 // ------------------------------------------------------------------ programmatic dependent launch (PDL)
 // A denoise step is a chain of ~1 400 short kernels; with the launch attribute below a kernel of this library may be scheduled
-// while its predecessor in the stream is still draining, run its prologue (TMEM / barrier set-up, tensor-map prefetch, index
+// while its predecessor in the stream is still draining, run its prologue (barrier set-up, tensor-map prefetch, index
 // arithmetic) and then block in pdl_wait() until the predecessor has completed and flushed its writes.  No global memory is
 // read or written before pdl_wait().  Opt-in per kernel family with the DF_PDL bit mask (without the attribute the device-side wait
 // is a no-op).

@@ -52,7 +52,7 @@ extern "C" int df_geglu(const void* in, void* out, int64_t rows, int cols, int64
   if (rows == 0) return 0;
   const int64_t total = rows * (cols / 8);
   int64_t g = (total + 255) / 256;
-  if (g > 148 * 16) g = 148 * 16;
+  if (g > kSmCount * 16) g = kSmCount * 16;
   DF_CHECK_CUDA(launch_pdl(PDL_ELEM, geglu_kernel, dim3((unsigned)g), dim3(256), 0, (cudaStream_t)stream, (const __half*)in, (__half*)out, rows,
                            cols / 8, in_pitch, out_pitch, cols));
   return 0;
@@ -112,7 +112,7 @@ extern "C" int df_bias_residual_add(const void* a, const void* residual, const v
   if (rows == 0) return 0;
   const int64_t total = rows * (C / 8);
   int64_t g = (total + 256 * 4 - 1) / (256 * 4);
-  if (g > 148 * 8) g = 148 * 8;
+  if (g > kSmCount * 8) g = kSmCount * 8;
   DF_CHECK_CUDA(launch_pdl(PDL_ELEM, bias_residual_add_kernel, dim3((unsigned)g), dim3(256), 0, (cudaStream_t)stream, (const __half*)a,
                            (const __half*)residual, (const __half*)bias, (__half*)out, total, C / 8));
   return 0;

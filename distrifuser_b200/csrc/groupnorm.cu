@@ -38,7 +38,7 @@ inline GnPlan gn_plan(int b, int h, int w, int C) {
   int active = p.lanes * p.V;
   p.threads = (active + 31) / 32 * 32;
   int hw = h * w;
-  int want = (2 * 148 + b - 1) / b;                  // ~2 CTAs per SM over the batch
+  int want = (2 * kSmCount + b - 1) / b;                  // ~2 CTAs per SM over the batch
   int cap = hw / (p.lanes * 8);                      // >= 8 pixels per thread
   if (cap < 1) cap = 1;
   p.nchunk = want < cap ? want : cap;
@@ -468,7 +468,7 @@ __global__ void __launch_bounds__(512) gn_apply_kernel(const __half* __restrict_
 // that the last arriver bumps.  After the barrier each CTA folds the per-CTA partials of its own sample itself (G x nchunk
 // values from L2, a coalesced microsecond) and keeps (mean, rstd) in shared memory; the first design let the last CTA reduce
 // everything, write coef[] and only then release the grid -- 6 us of serial work plus a global round trip in front of the
-// normalise pass of all 296 CTAs (profiles/r2_gn_trace.txt).  Then each CTA normalises the pixels it has just read (L1 / L2
+// normalise pass of the whole grid.  Then each CTA normalises the pixels it has just read (L1 / L2
 // hits: one HBM read and one write per element, one launch instead of two).  Exchange modes: the last arriver also publishes
 // this rank's statistics to the patch group (synchronous mode: before anything else -- the peers wait for them).
 __global__ void __launch_bounds__(512, 2) gn_fused_kernel(const __half* __restrict__ x, const __half* __restrict__ addend, int64_t addend_pitch,
@@ -578,7 +578,7 @@ int groupnorm_impl(df_comm_t comm, const void* x, const void* addend, int64_t ad
     const size_t need = (size_t)(2 * (groups * tpp + groups) + groups) * sizeof(float2);
     if (smem < need) smem = need;
   }
-  // one launch when the whole grid is resident at once (always, for the plans of gn_plan on a B200: <= 2 CTAs per SM)
+  // one launch when the whole grid is resident at once (always, for the plans of gn_plan on an H100: <= 2 CTAs per SM)
   static int fused_capacity = -1;
   if (fused_capacity < 0) {
     int dev = 0, sms = 0, per_sm = 0;

@@ -98,7 +98,7 @@ extern "C" int df_halo_assemble(df_comm_t comm, const void* x, void* xp, int b, 
              "df_halo_assemble: rows must be 16-byte multiples");
   uint64_t total = (uint64_t)b * (h + 2) * (row_bytes / 16);
   uint64_t g = (total + 256 * 8 - 1) / (256 * 8);
-  int grid = (int)(g < 1 ? 1 : (g > 148 * 8 ? 148 * 8 : g));
+  int grid = (int)(g < 1 ? 1 : (g > kSmCount * 8 ? kSmCount * 8 : g));
   halo_assemble_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(comm, (const char*)x, (char*)xp, b, h, row_bytes / 16, idx,
                                                               tensor_off, slot_bytes, up_rank, down_rank, wait_flags);
   DF_CHECK_LAUNCH();

@@ -1,22 +1,22 @@
-// distrifuser_b200 -- Linear layers of the transformer blocks as a hand-written tcgen05 GEMM with fused epilogues
+// distrifuser_b200 -- Linear layers of the transformer blocks as a hand-written wgmma GEMM with fused epilogues
 // (SURVEY 8f N1: "fused Linear epilogues (to_kv -> comm slot, GEGLU)"; reference call sites distrifuser/modules/pp/attn.py:121-125,159
 // and the diffusers FeedForward the wrappers live in).
 //
-//   out[M, N] = A[M, K] . W[N, K]^T  (+ bias[N]) (+ residual[M, N])          fp16 in, fp32 accumulate in TMEM, fp16 out
-//   GEGLU:  out[M, N/2] = (A.Wh^T + bh) * gelu_erf(A.Wg^T + bg)  with the rows of W interleaved in blocks of 128
-//           (hidden block t | gate block t), so that one 256-column accumulator tile holds both halves of 128 outputs:
+//   out[M, N] = A[M, K] . W[N, K]^T  (+ bias[N]) (+ residual[M, N])          fp16 in, fp32 accumulate in registers, fp16 out
+//   GEGLU:  out[M, N/2] = (A.Wh^T + bh) * gelu_erf(A.Wg^T + bg)  with the rows of W interleaved in blocks of BN/2
+//           (hidden block t | gate block t), so that one BN-column accumulator tile holds both halves of BN/2 outputs:
 //           the [M, 8C] projection of diffusers' GEGLU is never written to HBM (saves 3 * M * 4C * 2 B of traffic per layer
 //           and the separate geglu kernel)
 //   publish: columns >= pub_col0 of the result are ALSO stored into slot(pub, idx, me) of every peer in `peer_mask`
 //           (fused q|k|v projection: the k|v columns go straight into the peers' arenas over NVLink -- replaces the
 //           enqueue copy, utils.py:187, and the separate publication kernel); the last CTA stamps the peers' flags.
 //
-// Kernel: persistent CTA PAIRS (cluster of 2, tcgen05 cta_group::2).  A pair owns 256 x 256 output tiles: each CTA TMA-loads
-// its own 128 rows of A and HALF (128 rows) of the W tile per 64-wide K block into a 6-stage SWIZZLE_128B ring, the pair
-// leader issues M=256 N=256 K=16 MMAs that read both CTAs' shared memory (each operand byte is fetched from L2 once per
-// pair), accumulators live in TMEM (2 x 256 columns: the epilogue of tile i overlaps the main loop of tile i+1).
-//   warp 0    TMA producer (one lane)          warp 1    MMA issuer (one lane, leader CTA only)
-//   warps 2-9 epilogue (two per TMEM lane quarter, alternate 32-column chunks): tcgen05.ld 32 columns at a time -> bias / residual / GEGLU -> fp16 -> 16-byte global stores
+// Kernel: persistent CTAs, one per SM, each owning 128 x BN output tiles (BN = 256, or 160 where that fills the SMs better).
+// Per 64-wide K block the producer TMA-loads 128 rows of A and BN rows of W into a SWIZZLE_128B ring; two consumer warpgroups
+// each issue m64nBNk16 wgmmas for their 64 rows with the fp32 accumulators in registers, release the stage once the wgmma that
+// read it has retired, and run the epilogue straight from the accumulator fragment.  The producer keeps loading the next tile's
+// K blocks while the consumers are in the epilogue.
+//   warps 0-7  two consumer warpgroups (rows 0-63, 64-127 of the tile)      warp 8   TMA producer (one lane)
 #include <math.h>
 #include <string.h>
 
@@ -27,22 +27,21 @@ using namespace df::tc;
 
 namespace {
 
-constexpr int BM = 128;            // rows of A per CTA (256 per pair)
-// BN = output-tile columns (W rows) of a pair; each CTA stages BN/2 of them.  256 for large N and the GEGLU epilogue; 160 where 256
-// would leave most pairs idle (N = 1280 with M = 2048: 40 tiles on 74 pairs -> 64 tiles).  UMMA: M = 256 needs N % 16 == 0.
+constexpr int BM = 128;            // rows of A per tile (64 per consumer warpgroup)
 constexpr int BK = 64;             // one 128-byte swizzled row of fp16
-constexpr int STAGES = 6;
-constexpr int NTHREADS = 320;        // warp 0 TMA, warp 1 MMA, warps 2-9 epilogue (two per TMEM lane quarter)
-constexpr int NEPI_WARPS = 8;
+constexpr int NTHREADS = 288;      // warps 0-7: two consumer warpgroups, warp 8: TMA producer
+constexpr int NCONSUMER_WARPS = 8;
 constexpr uint32_t A_BYTES = BM * BK * 2;
+
+// BN = output-tile columns (W rows): 256 for large N and the GEGLU epilogue, 160 where 256 would leave SMs idle.  Stages: as
+// many as fit next to each other in the 227 KiB a block may use.
+template <int BN> struct Stages { static constexpr int value = BN == 256 ? 4 : 5; };
 
 template <int BN>
 struct __align__(1024) SmemT {
-  __half a[STAGES][BM * BK];
-  __half b[STAGES][(BN / 2) * BK];         // (BN / 2) * 128 B per stage: a multiple of 1 KiB for BN in {160, 256}
-  uint64_t full[STAGES], empty[STAGES];
-  uint64_t tmem_full[2], tmem_empty[2];
-  uint32_t tmem_base;
+  __half a[Stages<BN>::value][BM * BK];
+  __half b[Stages<BN>::value][BN * BK];      // BN * 128 B per stage: a multiple of 1 KiB for BN in {160, 256}
+  uint64_t full[Stages<BN>::value], empty[Stages<BN>::value];
 };
 
 enum { EPI_PLAIN = 0, EPI_GEGLU = 1 };
@@ -76,198 +75,119 @@ __device__ __forceinline__ float gelu_erf(float x) {      // same approximation 
   return x * phi;
 }
 
-__device__ __forceinline__ void unpack8h(const int4& v, float* f) {
-  const __half2* h = reinterpret_cast<const __half2*>(&v);
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    float2 t = __half22float2(h[i]);
-    f[2 * i] = t.x;
-    f[2 * i + 1] = t.y;
-  }
+__device__ __forceinline__ float2 ld_h2f(const __half* p) { return __half22float2(*reinterpret_cast<const __half2*>(p)); }
+
+template <int BN>
+__device__ __forceinline__ void wgmma_tile(float* acc, uint64_t a_desc, uint64_t b_desc, uint32_t accumulate) {
+  if constexpr (BN == 256) wgmma_ss_n256(acc, a_desc, b_desc, accumulate);
+  else wgmma_ss_n160(acc, a_desc, b_desc, accumulate);
 }
 
 template <int EPI, int BN>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(NTHREADS, 1)
+__global__ void __launch_bounds__(NTHREADS, 1)
 linear_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant__ CUtensorMap tm_w, LinearArgs p) {
-  static_assert(BN % 32 == 0 && BN <= 256 && ((BN / 2) * BK * 2) % 1024 == 0, "tile shape");
-  constexpr uint32_t B_BYTES = (BN / 2) * BK * 2;
-  constexpr uint32_t IDESC = (1u << 4) | ((uint32_t)(BN >> 3) << 17) | ((uint32_t)((2 * BM) >> 4) << 24);   // f16 x f16 -> f32, K-major A and B
+  static_assert(BN % 32 == 0 && BN <= 256 && (BN * BK * 2) % 1024 == 0, "tile shape");
+  constexpr int STAGES = Stages<BN>::value;
+  constexpr uint32_t B_BYTES = BN * BK * 2;
   using Smem = SmemT<BN>;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   Smem& sm = *reinterpret_cast<Smem*>(smem_raw);
   if ((smem_u32(smem_raw) & 1023u) != 0) __trap();
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_ctarank();                 // 0 = pair leader
-  const int pair = blockIdx.x >> 1, npairs = gridDim.x >> 1;
   const int ntiles = p.tiles_m * p.tiles_n;
   const int kblocks = p.K / BK;
 
-  if (warp == 1 && lane == 0) {
-    for (int s = 0; s < STAGES; ++s) { mbar_init(&sm.full[s], 1); mbar_init(&sm.empty[s], 1); }
-    for (int b = 0; b < 2; ++b) { mbar_init(&sm.tmem_full[b], 1); mbar_init(&sm.tmem_empty[b], 2 * NEPI_WARPS); }   // both CTAs' epilogue warps
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < STAGES; ++s) { mbar_init(&sm.full[s], 1); mbar_init(&sm.empty[s], NCONSUMER_WARPS); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&sm.tmem_base)), "r"(512u) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  cluster_sync_all();                                      // the peer's barriers exist before anything signals them
-  tc_fence_after();
-  const uint32_t tmem = sm.tmem_base;
   pdl_wait();                                              // set-up above overlapped the tail of the previous kernel
 
-  if (warp == 0) {
-    // =============================================================== TMA producer (both CTAs)
+  if (warp == NCONSUMER_WARPS) {
+    // =============================================================== TMA producer
     if (lane == 0) {
       prefetch_tmap(&tm_a);
       prefetch_tmap(&tm_w);
       uint32_t stage = 0, phase = 0;
-      for (int tile = pair; tile < ntiles; tile += npairs) {
+      for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
         const int tm = tile % p.tiles_m, tn = tile / p.tiles_m;
-        const int row0 = tm * (2 * BM) + (int)rank * BM, col0 = tn * BN + (int)rank * (BN / 2);
         for (int kb = 0; kb < kblocks; ++kb) {
           mbar_wait(&sm.empty[stage], phase ^ 1u);
-          if (rank == 0) mbar_expect_tx(&sm.full[stage], 2 * (A_BYTES + B_BYTES));
-          const uint32_t bar = mapa_u32(smem_u32(&sm.full[stage]), 0);       // the leader's barrier collects both CTAs' bytes
-          tma_load_2d_pair(sm.a[stage], &tm_a, bar, kb * BK, row0);
-          tma_load_2d_pair(sm.b[stage], &tm_w, bar, kb * BK, col0);
+          mbar_expect_tx(&sm.full[stage], A_BYTES + B_BYTES);
+          tma_load_2d(sm.a[stage], &tm_a, &sm.full[stage], kb * BK, tm * BM);
+          tma_load_2d(sm.b[stage], &tm_w, &sm.full[stage], kb * BK, tn * BN);
           if (++stage == STAGES) { stage = 0; phase ^= 1u; }
         }
-      }
-    }
-  } else if (warp == 1) {
-    // =============================================================== MMA issuer (leader CTA, one lane)
-    if (rank == 0 && lane == 0) {
-      uint32_t stage = 0, phase = 0;
-      int it = 0;
-      for (int tile = pair; tile < ntiles; tile += npairs, ++it) {
-        const uint32_t buf = (uint32_t)it & 1u, use = (uint32_t)it >> 1;
-        mbar_wait(&sm.tmem_empty[buf], (use & 1u) ^ 1u);   // both CTAs' epilogue warps drained this accumulator
-        tc_fence_after();
-        const uint32_t d = tmem + buf * BN;
-        for (int kb = 0; kb < kblocks; ++kb) {
-          mbar_wait(&sm.full[stage], phase);
-          tc_fence_after();
-          const uint32_t a_addr = smem_u32(sm.a[stage]), b_addr = smem_u32(sm.b[stage]);
-#pragma unroll
-          for (int kk = 0; kk < BK / 16; ++kk)
-            mma_ss_pair(d, smem_desc(a_addr + kk * 32, 16, 1024), smem_desc(b_addr + kk * 32, 16, 1024), IDESC, (kb | kk) > 0);
-          tc_commit_pair(&sm.empty[stage], 0x3);           // frees the stage in BOTH CTAs
-          if (++stage == STAGES) { stage = 0; phase ^= 1u; }
-        }
-        tc_commit_pair(&sm.tmem_full[buf], 0x3);
       }
     }
   } else {
-    // =============================================================== epilogue (warps 2-9 of both CTAs)
-    // warps w and w + 4 share a TMEM lane quarter (hardware: warp % 4) and take alternate 32-column chunks of the tile: with
-    // one warp per quarter the GEGLU epilogue (~40 instructions per output) took as long as the main loop of the next tile
-    const int quad = warp & 3;                             // TMEM lane quarter this warp may access
-    const int chalf = (warp - 2) >> 2;                     // 0: even chunks, 1: odd chunks
-    const int row = quad * 32 + lane;
-    const uint32_t lane_base = tmem + ((uint32_t)(quad * 32) << 16);
-    const uint32_t empty_bar0 = mapa_u32(smem_u32(&sm.tmem_empty[0]), 0), empty_bar1 = mapa_u32(smem_u32(&sm.tmem_empty[1]), 0);
+    // =============================================================== consumers (warps 0-7): main loop + epilogue
+    const int wg = warp >> 2;
+    const int c4 = lane & 3;
+    const int rloc = wg * 64 + (warp & 3) * 16 + (lane >> 2);   // tile row of accumulator rows A (rloc) and B (rloc + 8)
     uint32_t pub_epoch = 0;
     if (p.publish) pub_epoch = p.comm.clock[0];
-    int it = 0;
-    for (int tile = pair; tile < ntiles; tile += npairs, ++it) {
+    uint32_t stage = 0, phase = 0;
+    float acc[BN / 2];
+    for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
       const int tm = tile % p.tiles_m, tn = tile / p.tiles_m;
-      const uint32_t buf = (uint32_t)it & 1u, use = (uint32_t)it >> 1;
-      const int64_t grow = (int64_t)tm * (2 * BM) + (int64_t)rank * BM + row;
-      const bool row_ok = grow < p.M;
-      mbar_wait(&sm.tmem_full[buf], use & 1u);
-      tc_fence_after();
-      const uint32_t acc = lane_base + buf * BN;
-      if (EPI == EPI_GEGLU) {
-        // accumulator columns [0, BN/2) = hidden, [BN/2, BN) = gate of output columns [tn*BN/2, (tn+1)*BN/2); 16-column chunks
-        // (BN/2 = 80 or 128), alternate chunks per warp of a lane quarter
-        const int ocol0 = tn * (BN / 2);
-        __half* dst = p.out + grow * p.ldo + ocol0;
-#pragma unroll 1
-        for (int c = chalf * 16; c < BN / 2; c += 32) {
-          uint32_t h[16], g[16];
-          tmem_ld16(acc + c, h);
-          tmem_ld16(acc + BN / 2 + c, g);
-          tmem_wait_ld();
-          if (c + 32 >= BN / 2) {                          // this warp's last chunk is in registers: hand the accumulator back
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive_cluster(buf ? empty_bar1 : empty_bar0);
+      fence_regs<BN / 2>(acc);
+      uint32_t prev = 0;
+      for (int kb = 0; kb < kblocks; ++kb) {
+        mbar_wait(&sm.full[stage], phase);
+        const uint32_t a_addr = smem_u32(sm.a[stage]) + wg * 64 * 128, b_addr = smem_u32(sm.b[stage]);
+        wgmma_fence();
+#pragma unroll
+        for (int kk = 0; kk < BK / 16; ++kk)
+          wgmma_tile<BN>(acc, smem_desc(a_addr + kk * 32, 16, 1024), smem_desc(b_addr + kk * 32, 16, 1024), (kb | kk) > 0);
+        wgmma_commit();
+        wgmma_wait<1>();                                   // the previous K block's wgmmas have retired: its stage is free
+        if (kb > 0 && lane == 0) mbar_arrive(&sm.empty[prev]);
+        prev = stage;
+        if (++stage == STAGES) { stage = 0; phase ^= 1u; }
+      }
+      wgmma_wait<0>();
+      fence_regs<BN / 2>(acc);
+      if (lane == 0) mbar_arrive(&sm.empty[prev]);
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {                        // accumulator rows A / B of this thread
+        const int64_t grow = (int64_t)tm * BM + rloc + 8 * h;
+        if (grow >= p.M) continue;
+        if (EPI == EPI_GEGLU) {
+          // accumulator columns [0, BN/2) = hidden, [BN/2, BN) = gate of output columns [tn*BN/2, (tn+1)*BN/2); N % BN == 0
+          __half* dst = p.out + grow * p.ldo + tn * (BN / 2);
+#pragma unroll
+          for (int i = 0; i < BN / 16; ++i) {
+            const int c = 8 * i + 2 * c4;
+            float2 bh = make_float2(0.f, 0.f), bg = make_float2(0.f, 0.f);
+            if (p.bias) { bh = ld_h2f(p.bias + tn * BN + c); bg = ld_h2f(p.bias + tn * BN + BN / 2 + c); }
+            const float* hv = acc + 4 * i + 2 * h;
+            const float* gv = acc + 4 * (i + BN / 16) + 2 * h;
+            // diffusers rounds the projection to fp16 before hidden * gelu(gate): reproduce that rounding
+            const float2 hf = __half22float2(__floats2half2_rn(hv[0] + bh.x, hv[1] + bh.y));
+            const float2 gf = __half22float2(__floats2half2_rn(gv[0] + bg.x, gv[1] + bg.y));
+            *reinterpret_cast<__half2*>(dst + c) = __floats2half2_rn(hf.x * gelu_erf(gf.x), hf.y * gelu_erf(gf.y));
           }
-          if (row_ok) {
+        } else {
+          const int col0 = tn * BN;
+          __half* dst = p.out + grow * p.ldo + col0;
+          const __half* res = p.residual ? p.residual + grow * p.ldr + col0 : nullptr;
 #pragma unroll
-            for (int v = 0; v < 2; ++v) {
-              float bh[8], bg[8];
-              if (p.bias) {
-                unpack8h(ld_v4(p.bias + tn * BN + c + v * 8), bh);
-                unpack8h(ld_v4(p.bias + tn * BN + BN / 2 + c + v * 8), bg);
-              } else {
-#pragma unroll
-                for (int j = 0; j < 8; ++j) bh[j] = bg[j] = 0.f;
-              }
-              int4 o;
-              __half2* o2 = reinterpret_cast<__half2*>(&o);
-#pragma unroll
-              for (int j = 0; j < 4; ++j) {
-                const float h0 = __uint_as_float(h[v * 8 + 2 * j]) + bh[2 * j], h1 = __uint_as_float(h[v * 8 + 2 * j + 1]) + bh[2 * j + 1];
-                const float g0 = __uint_as_float(g[v * 8 + 2 * j]) + bg[2 * j], g1 = __uint_as_float(g[v * 8 + 2 * j + 1]) + bg[2 * j + 1];
-                // diffusers rounds the projection to fp16 before hidden * gelu(gate): reproduce that rounding
-                const __half2 hh = __floats2half2_rn(h0, h1), gg = __floats2half2_rn(g0, g1);
-                const float2 hf = __half22float2(hh), gf = __half22float2(gg);
-                o2[j] = __floats2half2_rn(hf.x * gelu_erf(gf.x), hf.y * gelu_erf(gf.y));
-              }
-              st_v4(dst + c + v * 8, o);                   // N % BN == 0: every column of the tile exists
-            }
-          }
-        }
-      } else {
-        const int col0 = tn * BN;
-        __half* dst = p.out + grow * p.ldo + col0;
-        const __half* res = p.residual ? p.residual + grow * p.ldr + col0 : nullptr;
-#pragma unroll 1
-        for (int c = chalf * 32; c < BN; c += 64) {
-          uint32_t acc_r[32];
-          tmem_ld32(acc + c, acc_r);
-          tmem_wait_ld();
-          if (c + 64 >= BN) {                              // this warp's last chunk
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive_cluster(buf ? empty_bar1 : empty_bar0);
-          }
-          if (row_ok && col0 + c < p.N) {
-#pragma unroll
-            for (int v = 0; v < 4; ++v) {
-              const int col = col0 + c + v * 8;
-              if (col < p.N) {                            // N % 8 == 0: a vector is entirely inside or outside
-                float f[8];
-#pragma unroll
-                for (int j = 0; j < 8; ++j) f[j] = __uint_as_float(acc_r[v * 8 + j]);
-                if (p.bias) {
-                  float bb[8];
-                  unpack8h(ld_v4(p.bias + col), bb);
-#pragma unroll
-                  for (int j = 0; j < 8; ++j) f[j] += bb[j];
-                }
-                int4 o;
-                __half2* o2 = reinterpret_cast<__half2*>(&o);
-#pragma unroll
-                for (int j = 0; j < 4; ++j) o2[j] = __floats2half2_rn(f[2 * j], f[2 * j + 1]);
-                if (res) {                                // torch: linear output rounded to fp16, then `+ residual` in fp16
-                  const int4 rv = ld_nc_v4(res + c + v * 8);
-                  const __half2* r2 = reinterpret_cast<const __half2*>(&rv);
-#pragma unroll
-                  for (int j = 0; j < 4; ++j) o2[j] = __hadd2(o2[j], r2[j]);
-                }
-                st_v4(dst + c + v * 8, o);
-                if (p.publish && col >= p.pub_col0) {     // k|v columns: also into every peer's slot of the publish epoch
-                  const uint64_t off = (uint64_t)(pub_epoch % DF_NBANKS) * p.comm.bank_stride + p.tensor_off +
-                                       (uint64_t)p.comm.rank * p.slot_bytes + ((uint64_t)grow * p.pub_cols + (col - p.pub_col0)) * 2;
-                  for (int q = 0; q < p.comm.world; ++q)
-                    if (p.peer_mask >> q & 1) st_v4((char*)p.comm.base[q] + off, o);
-                }
-              }
+          for (int i = 0; i < BN / 8; ++i) {
+            const int c = 8 * i + 2 * c4;
+            const int col = col0 + c;
+            if (col >= p.N) continue;                      // N % 8 == 0: a column pair is entirely inside or outside
+            float2 f = make_float2(acc[4 * i + 2 * h], acc[4 * i + 2 * h + 1]);
+            if (p.bias) { const float2 bb = ld_h2f(p.bias + col); f.x += bb.x; f.y += bb.y; }
+            __half2 o = __floats2half2_rn(f.x, f.y);
+            if (res) o = __hadd2(o, *reinterpret_cast<const __half2*>(res + c));   // torch: fp16 linear output, then fp16 add
+            *reinterpret_cast<__half2*>(dst + c) = o;
+            if (p.publish && col >= p.pub_col0) {          // k|v columns: also into every peer's slot of the publish epoch
+              const uint64_t off = (uint64_t)(pub_epoch % DF_NBANKS) * p.comm.bank_stride + p.tensor_off +
+                                   (uint64_t)p.comm.rank * p.slot_bytes + ((uint64_t)grow * p.pub_cols + (col - p.pub_col0)) * 2;
+              for (int q = 0; q < p.comm.world; ++q)
+                if (p.peer_mask >> q & 1) *reinterpret_cast<__half2*>((char*)p.comm.base[q] + off) = o;
             }
           }
         }
@@ -275,7 +195,6 @@ linear_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant__ 
     }
     if (p.publish) __threadfence_system();                 // peer stores of this thread are visible system-wide before the ticket
   }
-  tc_fence_before();
   __syncthreads();
   if (p.publish && threadIdx.x == 0) {
     // last CTA of the grid stamps the peers' flags (same protocol as publish_kernel, csrc/comm.cu)
@@ -288,10 +207,6 @@ linear_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant__ 
       for (int q = 0; q < p.comm.world; ++q)
         if (p.peer_mask >> q & 1) st_release_sys(p.comm.flags[q] + (size_t)p.idx * p.comm.world + p.comm.rank, epoch);
     }
-  }
-  cluster_sync_all();                                      // the peer may still be signalling this CTA's barriers / reading its smem
-  if (warp == 0) {
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(512u) : "memory");
   }
 }
 
@@ -333,20 +248,17 @@ int launch_linear(const CUtensorMap& ta, const CUtensorMap& tw, const LinearArgs
     DF_CHECK_CUDA(cudaFuncSetAttribute(linear_kernel<EPI, BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(SmemT<BN>)));
     attr_set = true;
   }
-  DF_CHECK_CUDA(launch_pdl(PDL_GEMM, linear_kernel<EPI, BN>, dim3(ctas), dim3(NTHREADS), sizeof(SmemT<BN>), st, ta, tw, args));   // cluster of 2: __cluster_dims__
+  DF_CHECK_CUDA(launch_pdl(PDL_GEMM, linear_kernel<EPI, BN>, dim3(ctas), dim3(NTHREADS), sizeof(SmemT<BN>), st, ta, tw, args));
   return 0;
 }
 
-// Relative cost of a problem with pair tiles of width bn: rounds x cycles per 64-wide K block of one tile.  A K block costs
-// max(tensor cycles, shared-memory cycles): 2*bn cycles of M=256 MMAs against (16 KiB of A + bn*64 B of W) written by TMA AND
-// read by the tensor core through a 128 B/cycle port = 256 + bn cycles.  256-wide tiles balance the two (512 / 512); 160-wide
-// tiles are shared-memory bound (320 / 416) and only pay off when they fill many more pairs (measured: the 2048 x 10240 GEGLU
-// projection runs 49 us with 256-wide and 52 us with 160-wide tiles although the latter waste no round -- profiles/r2_linear_*).
-double tile_cost(int64_t M, int N, int bn, int pairs_avail) {
-  const long long tm = (M + 2 * BM - 1) / (2 * BM), tn = (N + bn - 1) / bn, tiles = tm * tn;
-  const long long rounds = (tiles + pairs_avail - 1) / pairs_avail;
-  const int per_kblock = 2 * bn > 256 + bn ? 2 * bn : 256 + bn;
-  return (double)rounds * per_kblock;
+// Relative cost of a problem with 128 x bn tiles: rounds x cycles per 64-wide K block of one tile.  The wgmmas of a K block take
+// time proportional to bn, while the A half of the operand traffic (16 KiB per K block) is paid whatever bn is: a 160-wide tile
+// moves 36 KiB for 160 columns, a 256-wide one 48 KiB for 256, so narrow tiles only pay off when they fill clearly more SMs.
+double tile_cost(int64_t M, int N, int bn, int ctas_avail) {
+  const long long tm = (M + BM - 1) / BM, tn = (N + bn - 1) / bn, tiles = tm * tn;
+  const long long rounds = (tiles + ctas_avail - 1) / ctas_avail;
+  return (double)rounds * (bn + 64);
 }
 
 }  // namespace
@@ -354,10 +266,10 @@ double tile_cost(int64_t M, int N, int bn, int pairs_avail) {
 namespace {
 int sm_count_cached() {
   static int sms = 0;
-  if (!sms) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev); if (sms <= 0) sms = 148; }
+  if (!sms) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev); if (sms <= 0) sms = kSmCount; }
   return sms;
 }
-// pair-tile width for a problem: 256, or 160 where that fills the pairs better (GEGLU: only widths that tile N exactly)
+// tile width for a problem: 256, or 160 where that fills the SMs better (GEGLU: only widths that tile N exactly)
 int pick_bn(int64_t M, int N, int epilogue, int cap) {
   const bool ok160 = epilogue == EPI_PLAIN || N % 160 == 0, ok256 = epilogue == EPI_PLAIN || N % 256 == 0;
   if (!ok256) return ok160 ? 160 : 0;
@@ -368,14 +280,14 @@ int pick_bn(int64_t M, int N, int epilogue, int cap) {
 
 extern "C" int df_linear_supported(int64_t M, int N, int K, int epilogue) {
   if (M < 1 || N < 8 || N % 8 != 0 || K < BK || K % BK != 0) return 0;
-  if (epilogue == EPI_GEGLU && pick_bn(M, N, epilogue, sm_count_cached() / 2) == 0) return 0;   // blocks of 80 / 128 must tile N / 2
+  if (epilogue == EPI_GEGLU && pick_bn(M, N, epilogue, sm_count_cached()) == 0) return 0;   // blocks of 80 / 128 must tile N / 2
   return 1;
 }
 
-// GEGLU epilogue: rows of the interleaved weight per hidden / gate block (= half the pair-tile width chosen for this problem)
+// GEGLU epilogue: rows of the interleaved weight per hidden / gate block (= half the tile width chosen for this problem)
 extern "C" int df_linear_geglu_block(int64_t M, int N, int K) {
   (void)K;
-  const int bn = pick_bn(M, N, EPI_GEGLU, sm_count_cached() / 2);
+  const int bn = pick_bn(M, N, EPI_GEGLU, sm_count_cached());
   return bn / 2;
 }
 
@@ -395,14 +307,14 @@ extern "C" int df_linear_fwd(df_comm_t comm, const void* a, const void* w, const
   args.bias = (const __half*)bias; args.residual = (const __half*)residual; args.out = (__half*)out;
   args.M = M; args.N = N; args.K = K; args.ldr = ldr; args.ldo = ldo;
   const int sms = sm_count_cached();
-  const int cap = (max_ctas > 0 ? max_ctas : sms) / 2 > 0 ? (max_ctas > 0 ? max_ctas : sms) / 2 : 1;
-  int bn = pick_bn(M, N, epilogue, epilogue == EPI_GEGLU ? sms / 2 : cap);   // GEGLU: must agree with df_linear_geglu_block()
+  const int cap = max_ctas > 0 ? max_ctas : sms;
+  int bn = pick_bn(M, N, epilogue, epilogue == EPI_GEGLU ? sms : cap);   // GEGLU: must agree with df_linear_geglu_block()
   if (epilogue == EPI_GEGLU && geglu_block > 0) {
     DF_REQUIRE(geglu_block == 80 || geglu_block == 128, "df_linear_fwd: geglu_block must be 80 or 128");
     bn = 2 * geglu_block;
     DF_REQUIRE(N % bn == 0, "df_linear_fwd: interleave block %d does not tile N=%d", geglu_block, N);
   }
-  args.tiles_m = (int)((M + 2 * BM - 1) / (2 * BM));
+  args.tiles_m = (int)((M + BM - 1) / BM);
   args.tiles_n = (N + bn - 1) / bn;
   args.publish = publish && peer_mask != 0;
   args.comm = comm;
@@ -412,17 +324,17 @@ extern "C" int df_linear_fwd(df_comm_t comm, const void* a, const void* w, const
     args.tensor_off = tensor_off; args.slot_bytes = slot_bytes;
     DF_REQUIRE((uint64_t)M * args.pub_cols * 2 <= slot_bytes, "df_linear_fwd: published columns larger than the slot");
   }
-  int pairs = args.tiles_m * args.tiles_n;
-  if (pairs > cap) pairs = cap;
-  if (pairs < 1) pairs = 1;
+  int ctas = args.tiles_m * args.tiles_n;
+  if (ctas > cap) ctas = cap;
+  if (ctas < 1) ctas = 1;
   CUtensorMap ta, tw;
   if (int rc = make_map2d(&ta, a, M, K, lda, BM)) return rc;
-  if (int rc = make_map2d(&tw, w, N, K, ldw, bn / 2)) return rc;
+  if (int rc = make_map2d(&tw, w, N, K, ldw, bn)) return rc;
   cudaStream_t st = (cudaStream_t)stream;
   if (epilogue == EPI_GEGLU) {
-    if (bn == 160) return launch_linear<EPI_GEGLU, 160>(ta, tw, args, 2 * pairs, st);
-    return launch_linear<EPI_GEGLU, 256>(ta, tw, args, 2 * pairs, st);
+    if (bn == 160) return launch_linear<EPI_GEGLU, 160>(ta, tw, args, ctas, st);
+    return launch_linear<EPI_GEGLU, 256>(ta, tw, args, ctas, st);
   }
-  if (bn == 160) return launch_linear<EPI_PLAIN, 160>(ta, tw, args, 2 * pairs, st);
-  return launch_linear<EPI_PLAIN, 256>(ta, tw, args, 2 * pairs, st);
+  if (bn == 160) return launch_linear<EPI_PLAIN, 160>(ta, tw, args, ctas, st);
+  return launch_linear<EPI_PLAIN, 256>(ta, tw, args, ctas, st);
 }

@@ -3,7 +3,7 @@
 Same constructor, forward signature (including the non-diffusers `record` kwarg), counter protocol, CFG batch
 split and three-graph replay as the reference.  Differences, all internal:
   * the wrappers are installed for every world size (the reference leaves world_size==1 unwrapped, :18), so the
-    sm_100a kernels are the only attention / GroupNorm path;
+    sm_90a kernels are the only attention / GroupNorm path;
   * the final epsilon all_gather + cat (:162-169,186-193) is df_output_gather: each rank stores its strip into
     every peer's arena and waits on flags;
   * GroupNorm -> SiLU pairs of ResnetBlock2D / conv_norm_out run fused inside the GroupNorm kernel.

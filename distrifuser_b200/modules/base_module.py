@@ -56,7 +56,7 @@ class BaseModule(nn.Module):
     def set_comm_manager(self, comm_manager):
         self.comm_manager = comm_manager
 
-    # -- helpers shared by the B200 wrappers
+    # -- helpers shared by the native wrappers
     def _is_sync_step(self) -> bool:
         """counter <= warmup_steps  (attn.py:132, conv2d.py:92, groupnorm.py:45)."""
         return self.counter <= self.distri_config.warmup_steps

@@ -2,7 +2,7 @@
 
 q / fused kv / out projections stay library GEMMs (cuBLAS through F.linear); everything between them --
 the reference's torch.cat of the per-rank K/V (attn.py:131-138), split / view / transpose (:142-149) and
-F.scaled_dot_product_attention (:153) -- is one tcgen05 kernel (df_attn_fwd) that TMA-loads the K/V tiles
+F.scaled_dot_product_attention (:153) -- is one wgmma kernel (df_attn_fwd) that TMA-loads the K/V tiles
 straight from the n per-rank segments: this rank's fresh projection and the peers' 1-step-stale arena slots."""
 import ctypes as C
 import os
@@ -135,8 +135,7 @@ class DistriSelfAttentionPP(DistriAttentionPP):
         LoRA fuse/unfuse, in-place edits, .to()/.half()): the key holds the tensors' version counters and storage.
         Heads narrower than 64 (SD1.x level 0: d = 40) are stored 64 wide -- zero rows in the projection, zero columns in
         to_out, the softmax scale passed explicitly: an 80-byte head row at offset 80*h of the token row costs the TMA 1.6 cache
-        lines per row request and left the kernel waiting for K/V tiles (profiles/r2_attn_d40_tma_bound.txt); 128-byte rows
-        are one line each.  DF_PAD_HEADS=0 keeps the narrow layout."""
+        lines per row request and leaves the kernel waiting for K/V tiles; 128-byte rows are one line each.  DF_PAD_HEADS=0 keeps the narrow layout."""
         to_q, to_kv = self.module.to_q, self.to_kv
         if not (isinstance(to_q, nn.Linear) and to_q.bias is None and to_kv.bias is None and
                 to_q.in_features == to_kv.in_features and to_q.out_features * 2 == to_kv.out_features and
@@ -186,7 +185,7 @@ class DistriSelfAttentionPP(DistriAttentionPP):
         if w_qkv is not None:
             from ... import ops
             if not padded and ops.use_fused_linear("qkv") and ops.linear_supported(b * l, 3 * c, c):
-                # hand-written tcgen05 GEMM; its epilogue stores the k|v columns straight into the peers' arena slots and the
+                # hand-written wgmma GEMM; its epilogue stores the k|v columns straight into the peers' arena slots and the
                 # last CTA stamps their flags: no enqueue copy (utils.py:187), no separate publication kernel
                 pub = (cm.group, c, self.idx, cm.peers_mask(), cm.tensor_off[self.idx], cm.slot_bytes[self.idx]) if ship else None
                 qkv = ops.linear(hidden_states, w_qkv, publish=pub)

@@ -70,10 +70,11 @@ def conv2d_bias_residual(x: torch.Tensor, conv: torch.nn.Conv2d, padding, residu
     return out
 
 
-# ---------------------------------------------------------------------------------------------------- tcgen05 GEMM (csrc/linear.cu)
+# ---------------------------------------------------------------------------------------------------- wgmma GEMM (csrc/linear.cu)
 
 # which Linear layers run on the hand-written GEMM: comma list out of {geglu, qkv, out, ff2, proj}; "all" / "none".
-# Default = the set measured faster than cuBLAS on B200 (tools/bench_linear.py, profiles/r2_linear_vs_cublas.txt).
+# Default: the GEGLU projection, whose fused epilogue saves the [M, 8C] intermediate; tools/bench_linear.py compares the rest
+# with cuBLAS at the model's shapes.
 _FUSED_LINEAR = set(_os.environ.get("DF_LINEAR", "geglu").replace("all", "geglu,qkv,out,ff2,proj").split(","))
 
 
@@ -89,8 +90,8 @@ def linear_supported(M: int, N: int, K: int, geglu: bool = False) -> bool:
 
 
 def geglu_block(M: int, two_d: int, K: int) -> int:
-    """Rows per hidden / gate block the fused kernel wants for this problem (80 or 128; 0 = not supported): half of the pair-tile
-    width, chosen so that the tiles fill the 74 CTA pairs (e.g. 2048 x 10240: 256-wide tiles leave 14 % of the last round idle)."""
+    """Rows per hidden / gate block the fused kernel wants for this problem (80 or 128; 0 = not supported): half of the tile
+    width, chosen so that the tiles fill the SMs (160-wide tiles where they need clearly fewer rounds than 256-wide ones)."""
     if not linear_supported(M, two_d, K, geglu=True):
         return 0
     return int(_lib.lib().df_linear_geglu_block(M, two_d, K))
@@ -112,7 +113,7 @@ def geglu_interleave(weight: torch.Tensor, bias: torch.Tensor | None, block: int
 
 def linear(x: torch.Tensor, weight: torch.Tensor, bias: torch.Tensor | None = None, residual: torch.Tensor | None = None,
            out: torch.Tensor | None = None, publish=None) -> torch.Tensor:
-    """x[..., K] @ weight[N, K]^T (+ bias) (+ residual) on the hand-written tcgen05 GEMM.  `publish` = (comm, pub_col0, idx,
+    """x[..., K] @ weight[N, K]^T (+ bias) (+ residual) on the hand-written wgmma GEMM.  `publish` = (comm, pub_col0, idx,
     peer_mask, tensor_off, slot_bytes): the columns >= pub_col0 also go into the peers' arena slots."""
     assert x.is_cuda and x.dtype == torch.float16 and weight.dtype == torch.float16 and x.stride(-1) == 1 and weight.stride(-1) == 1
     K = x.shape[-1]

@@ -54,8 +54,8 @@ class _DistriPipelineBase:
         assert cfg.height % 8 == 0 and cfg.width % 8 == 0
         static_inputs = self._static_inputs(**kwargs)
         unet = pipeline.unet
-        # cuDNN heuristics pick legacy sm80 "wo_smem" implicit-GEMM kernels for several 3x3 shapes on sm_100
-        # (profiles/r1_launches_1024.md); autotuning happens in the un-captured passes below
+        # cuDNN's default heuristics are not always the fastest 3x3 algorithm at these shapes; autotuning happens in the
+        # un-captured passes below
         torch.backends.cudnn.benchmark = True
         comm_manager = None
         # the reference creates the manager only for n_device_per_batch > 1 (pipelines.py:132); the final epsilon
@@ -90,7 +90,7 @@ class _DistriPipelineBase:
             # the compute kernels are captured on a stream of priority DF_COMPUTE_PRIO (default -1 = above the publication
             # stream's 0): when a K/V projection finishes, the attention grid that follows it takes the SM slots before the
             # publication kernel of the same K/V does -- a publication CTA that got there first keeps a persistent attention
-            # CTA out of its SM for the whole transfer (profiles/r2_exposed_comm_n8.txt)
+            # CTA out of its SM for the whole transfer
             prio = int(os.environ.get("DF_COMPUTE_PRIO", "-1" if cfg.n_device_per_batch > 1 else "0"))   # no publications without patch peers
             capture_stream = torch.cuda.Stream(device=cfg.device, priority=prio)
             for counter in counters:

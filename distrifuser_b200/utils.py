@@ -1,5 +1,5 @@
 """DistriConfig and PatchParallelismCommManager -- same names, constructor signatures and method names as the
-reference (distrifuser/utils.py:23-110 and :112-199); internals are B200-native.
+reference (distrifuser/utils.py:23-110 and :112-199); internals are H100-native.
 
 The reference ships activations with batched async NCCL all_gathers into one flat buffer per peer.  Here every
 rank owns a *symmetric arena* mapped into all peers with CUDA IPC (NVLink 5 / NVSwitch peer memory); producers
@@ -116,7 +116,7 @@ class DistriConfig:
             rank = self.rank
         return rank % self.n_device_per_batch
 
-    # -- additions used by the B200 path
+    # -- additions used by the native path
     def patch_group_ranks(self) -> list[int]:
         """World ranks of the patch group of this rank (the reference's batch_group, utils.py:87-90)."""
         n = self.n_device_per_batch
@@ -151,7 +151,7 @@ class PatchParallelismCommManager:
         self.starts, self.ends, self.shapes = [], [], []
         self.idx_queue = []
         self.handles = None
-        # B200 path state
+        # native path state
         self.slot_bytes: list[int] = []
         self.dtypes: list[torch.dtype] = []
         self.tensor_off: list[int] = []
@@ -334,7 +334,7 @@ class PatchParallelismCommManager:
         if num_ctas is None:
             # synchronous steps wait for the data right away: use the whole NVLink; asynchronous publication hides under the
             # attention that follows and should take few SM slots
-            num_ctas = int(os.environ.get("DF_PUB_CTAS", "64")) if async_stream else 296
+            num_ctas = int(os.environ.get("DF_PUB_CTAS", "64")) if async_stream else 2 * 132   # two CTAs per SM of an H100
         main = torch.cuda.current_stream()
         if async_stream:
             self.comm_stream.wait_stream(main)      # fork: publication overlaps the compute that follows

@@ -1,5 +1,5 @@
 /*
- * distrifuser_b200 -- C ABI of the B200-native patch-parallel UNet hot path.
+ * distrifuser_b200 -- C ABI of the H100-native patch-parallel UNet hot path.
  *
  * The reference (mit-han-lab/distrifuser) has no FFI: its "plugin API" is Python class substitution
  * (distrifuser/models/distri_sdxl_unet_pp.py:18-40).  Each entry point below replaces the torch / NCCL
@@ -172,7 +172,7 @@ int df_bias_residual_add(const void* a, const void* residual /* nullable */, con
 int df_add_layernorm(const void* x, const void* r, void* s_out, void* y, const void* gamma, const void* beta,
                      int64_t rows, int C, float eps, void* stream);
 
-/* ---- Linear layers of the transformer blocks as a tcgen05 GEMM with fused epilogues (SURVEY 8f N1; reference call sites
+/* ---- Linear layers of the transformer blocks as a wgmma GEMM with fused epilogues (SURVEY 8f N1; reference call sites
  *      distrifuser/modules/pp/attn.py:121-125,159 and the diffusers FeedForward between the wrappers):
  *        out[M,N] = a[M,K] . w[N,K]^T (+ bias[N]) (+ residual[M,N])                         epilogue 0
  *        out[M,N/2] = (a.Wh^T + bh) * gelu_erf(a.Wg^T + bg), rows of w (and bias) interleaved in blocks of
@@ -184,7 +184,7 @@ int df_add_layernorm(const void* x, const void* r, void* s_out, void* y, const v
  *      half of the fused q|k|v projection goes straight into the peers' arenas (replaces enqueue, utils.py:181-190).
  *      max_ctas: 0 = all SMs. ------------------------------------------------------------------------------- */
 int df_linear_supported(int64_t M, int N, int K, int epilogue);
-/* rows per hidden / gate block of the interleaved GEGLU weight for this problem (80 or 128 = half the pair-tile width the
+/* rows per hidden / gate block of the interleaved GEGLU weight for this problem (80 or 128 = half the tile width the
  * kernel will use); pass the same value as `geglu_block` (0 = let the kernel pick, must then match the interleave). */
 int df_linear_geglu_block(int64_t M, int N, int K);
 int df_linear_fwd(df_comm_t comm, const void* a, const void* w, const void* bias, const void* residual, void* out,

@@ -18,7 +18,7 @@ def align(x, a):
 
 
 class LoopbackArena:
-    """One process, one GPU: an arena whose `n` ranks all alias this rank's memory.  Lets a single B200 exercise the
+    """One process, one GPU: an arena whose `n` ranks all alias this rank's memory.  Lets a single GPU exercise the
     slot addressing, banks, flags and epoch clock of the multi-rank kernels; the test writes the "peers'" data and
     flags itself."""
 

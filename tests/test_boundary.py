@@ -28,13 +28,13 @@ def test_header_symbols_exported(libpath):
     assert sorted(_lib.EXPORTS) == declared
 
 
-def test_library_is_sm100a_tcgen05(libpath):
+def test_library_is_sm90a_wgmma(libpath):
     sass = subprocess.run(["cuobjdump", "-sass", libpath], capture_output=True, text=True).stdout
-    assert "sm_100a" in sass or "SM100" in sass.upper()
-    for mnemonic in ("UTCHMMA", "LDTM", "STTM", "UTMALDG"):
-        assert mnemonic in sass, f"{mnemonic} missing: the attention kernel is not a tcgen05/TMA kernel"
-    assert "UTCHMMA.2CTA" in sass, "the GEMM must issue CTA-pair (cta_group::2) tensor-core instructions"
-    assert "HMMA." not in sass.replace("UTCHMMA", ""), "legacy mma.sync tensor path in the library"
+    assert "sm_90a" in sass
+    for mnemonic in ("HGMMA.64x128x16", "HGMMA.64x64x16", "UTMALDG", "SYNCS"):
+        assert mnemonic in sass, f"{mnemonic} missing: the attention kernel is not a wgmma/TMA/mbarrier kernel"
+    assert "HGMMA.64x256x16" in sass, "the GEMM must issue 64x256 warpgroup MMAs"
+    assert "HMMA." not in sass, "legacy mma.sync tensor path in the library"
 
 
 def test_error_channel(libpath):

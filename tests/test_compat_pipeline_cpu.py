@@ -84,7 +84,7 @@ def test_launch_summarizer_families(tmp_path):
     assert "elementwise" in m.family("void at::vectorized_elementwise_kernel<8, at::CUDAFunctor_add<c10::Half>>")
     # cuDNN's sm100 convolutions are cutlass3x "... implicit_gemm_fprop ..." kernels: they must not be booked as cuBLAS (round-1 bug)
     assert m.family("cutlass3x_sm100_tensorop_s256x256x16implicit_gemm_fprop_f16_f16_f32_void_f16_...") == "library conv (cuDNN)"
-    assert m.family("void <unnamed>::linear_kernel<1, 256>(CUtensorMap_st, CUtensorMap_st, <unnamed>::LinearArgs)").startswith("OURS tcgen05 GEMM")
+    assert m.family("void <unnamed>::linear_kernel<1, 256>(CUtensorMap_st, CUtensorMap_st, <unnamed>::LinearArgs)").startswith("OURS wgmma GEMM")
     assert m.family("<unnamed>::gn_fused_kernel(const __half *, ...)").startswith("OURS gn_fused")
 
 

@@ -1,6 +1,6 @@
 """CPU check that the product's diffusers-compatible UNet (distrifuser_b200/compat) is the same function as the
 oracle's diffusers-0.24.0 restatement: identical state-dict keys / shapes / parameter counts and identical fp32
-outputs (attention is patched with plain SDPA here -- on the GPU it is always the tcgen05 kernel)."""
+outputs (attention is patched with plain SDPA here -- on the GPU it is always the wgmma kernel)."""
 import pytest
 import torch
 from torch.nn import functional as F

@@ -1,4 +1,4 @@
-"""GPU parity of each sm_100a kernel through the C ABI, against fp32 torch restatements of the reference math
+"""GPU parity of each sm_90a kernel through the C ABI, against fp32 torch restatements of the reference math
 (oracle/pp_modules.py for the mode formulas).  Tolerances are for fp16 storage with fp32 accumulation:
 attention 2e-3 abs on O(1) outputs (P is rounded to fp16 before PV, like every flash kernel), GroupNorm 4e-3
 (one fp16 rounding of the output), halo / publication bit-exact."""
@@ -44,13 +44,13 @@ def _attn(q, kv, heads, comm=None, maps=None, nseg=1, own=0, idx=0, lseg=None, w
     (1, 256, 8192, 4, 64),         # tiny grid, long K/V: 8 K/V parts per unit, merged in-kernel by the last arriver
     (1, 130, 4100, 3, 64),         # split-KV with ragged q and k/v tiles
     (1, 100, 3000, 2, 40),         # split-KV, zero-padded head dim
-    (2, 4096, 77, 10, 64),         # persistent CTAs: 640 one-tile work units on 296 resident CTAs (cross-attention at 1024^2 level 1)
+    (2, 4096, 77, 10, 64),         # persistent CTAs: 640 one-tile work units on 132 resident CTAs (cross-attention at 1024^2 level 1)
     (2, 2048, 300, 20, 64),        # persistent CTAs: 640 units x 3 tiles, ragged last tile
-    (2, 1100, 520, 8, 80),         # persistent CTAs, two head blocks, one CTA per SM: 144 units (< 148) and ragged q
-    (2, 2304, 260, 8, 160),        # persistent CTAs, three head blocks: 288 units on 148 CTAs
-    (2, 1024, 1024, 20, 64),       # SDXL 1024^2 level 2: 320 units on 296 CTAs (24 CTAs take a second unit)
-    (2, 4096, 1024, 10, 64),       # 640 units: two whole units per CTA + 48 left-over units
-    (1, 256, 2048, 20, 64),        # 40 units x 16 tiles on 296 slots: 2 K/V parts per unit, merged in-kernel by the last arriver
+    (2, 1100, 520, 8, 80),         # persistent CTAs, two head blocks: 144 units on 132 CTAs and ragged q
+    (2, 2304, 260, 8, 160),        # persistent CTAs, three head blocks: 288 units on 132 CTAs
+    (2, 1024, 1024, 20, 64),       # SDXL 1024^2 level 2: 320 units on 132 CTAs (56 CTAs take a third unit)
+    (2, 4096, 1024, 10, 64),       # 640 units: four whole units per CTA + 112 left-over units
+    (1, 256, 2048, 20, 64),        # 40 units x 16 tiles on 132 slots: 2 K/V parts per unit, merged in-kernel by the last arriver
     (1, 200, 3000, 3, 80),         # split units with two head blocks, ragged q and k/v
 ])
 def test_attention_single_segment(b, lq, lk, heads, d):
@@ -66,7 +66,7 @@ def test_attention_single_segment(b, lq, lk, heads, d):
 
 @pytest.mark.parametrize("b,lq,lk,heads,d,gain", [(2, 2048, 300, 20, 64, 1.0), (2, 1024, 1024, 20, 64, 30.0), (2, 1100, 520, 8, 80, 1.0)])
 def test_attention_static_schedule_without_workspace(b, lq, lk, heads, d, gain):
-    """No workspace: every CTA walks its static list of whole units (and replays the ones a large logit jump poisons)."""
+    """No workspace: every CTA walks its static list of whole units (one case with a large logit jump half-way)."""
     torch.manual_seed(3)
     Cq = heads * d
     q = torch.randn(b, lq, Cq, device="cuda", dtype=torch.float16) * (4 if gain > 1 else 1)
@@ -106,26 +106,26 @@ def test_attention_tail_split_is_planned():
     from distrifuser_b200 import _lib
     L = _lib.lib()
     HDR = 1024
-    assert L.df_attn_workspace_bytes(1, 256, 8192, 1, 4, 64) > HDR         # 8 units on 296 slots, 64 K/V tiles
-    assert L.df_attn_workspace_bytes(2, 1024, 1024, 1, 20, 64) == HDR      # 320 units fill the 296 slots: whole units, dynamic tickets
-    assert L.df_attn_workspace_bytes(1, 1024, 4096, 1, 10, 64) > HDR       # SDXL 1024^2 n=4 level 1: 80 units x 32 tiles -> 3 parts
+    assert L.df_attn_workspace_bytes(1, 256, 8192, 1, 4, 64) > HDR         # 8 units on 132 slots, 64 K/V tiles
+    assert L.df_attn_workspace_bytes(2, 1024, 1024, 1, 20, 64) == HDR      # 320 units fill the 132 slots: whole units, dynamic tickets
+    assert L.df_attn_workspace_bytes(1, 512, 4096, 1, 10, 64) > HDR        # SDXL 1024^2 n=8 level 1: 40 units x 32 tiles -> 3 parts
     assert L.df_attn_workspace_bytes(2, 1024, 77, 1, 20, 64) == HDR        # cross-attention: one K/V tile, nothing to cut
-    assert L.df_attn_workspace_bytes(1, 3600, 3600, 4, 20, 64) == HDR      # 580 units on 296 slots -> whole units
+    assert L.df_attn_workspace_bytes(1, 3600, 3600, 4, 20, 64) == HDR      # 580 units on 132 slots -> whole units
 
 
 @pytest.mark.parametrize("case", ["late_tiles_x6", "late_tiles_x40", "some_rows", "one_polynomial_column", "one_mufu_column",
                                   "ragged_then_large", "split_parts"])
 def test_attention_large_logits_rescale(case):
-    """Later K/V tiles whose logits exceed the first tile's by far more than the fp16 head-room of P: the speculative pass (stale
-    exponent reference, no row maxima) must notice and redo the tile with the maxima first, rescaling O and l.  The cases cover
-    every warp redoing, only the warps of some rows redoing, the overflow sitting in a single column that takes the polynomial
-    exp2 (exponent wrap-around at x >= 128) or the MUFU exp2, a ragged tile before the jump, and split K/V parts."""
+    """Later K/V tiles whose logits exceed the first tile's by far more than the fp16 head-room of P: the online softmax must
+    move the exponent reference and rescale O and l.  The cases cover every row moving, only the rows of one warp moving, the
+    jump sitting in a single column that takes the polynomial exp2 or the MUFU exp2, a ragged tile before the jump, and split
+    K/V parts."""
     torch.manual_seed(1)
     b, lq, lk, heads, d = 1, 128, 512, 1, 64
     if case == "ragged_then_large":
         lq, lk = 200, 777
     if case == "split_parts":
-        lq, lk, heads = 256, 4096, 2          # 4 units on 296 slots: K/V parts merged by the last arriver
+        lq, lk, heads = 256, 4096, 2          # 4 units on 132 slots: K/V parts merged by the last arriver
     q = torch.randn(b, lq, heads * d, device="cuda", dtype=torch.float16) * 4
     kv = torch.randn(b, lk, 2 * heads * d, device="cuda", dtype=torch.float16)
     C = heads * d

@@ -1,4 +1,4 @@
-"""GPU parity of the tcgen05 GEMM (csrc/linear.cu, df_linear_fwd) through the C ABI against fp32 torch restatements:
+"""GPU parity of the wgmma GEMM (csrc/linear.cu, df_linear_fwd) through the C ABI against fp32 torch restatements:
 plain / bias / bias+residual epilogues, the fused GEGLU epilogue (diffusers GEGLU.forward) and the fused publication of
 the k|v columns into the peers' arena slots.  Tolerance: fp16 storage of an fp32-accumulated result (|err| <= 2e-3 * |ref|
 + 2e-3 on O(1) data; K up to 5120)."""
@@ -17,12 +17,12 @@ def _close(out, ref, rel=2e-3, abs_=4e-3):
 
 
 @pytest.mark.parametrize("M,N,K", [
-    (256, 256, 64),            # one pair tile, one K block
+    (256, 256, 64),            # one tile row pair, one K block
     (2048, 1280, 1280),        # SDXL level-2 attention projections at 1024^2 (to_out / to_q)
     (2048, 3840, 1280),        # fused q|k|v projection
     (8192, 640, 640),          # level 1: N = 2.5 tiles (column tail)
-    (154, 2560, 2048),         # text K/V projection: 2 x 77 rows (row tail inside one pair tile)
-    (3600, 1280, 5120),        # 3840^2 n=4 level-2 FF2: ragged rows (3600 = 14 * 256 + 16), long K
+    (154, 2560, 2048),         # text K/V projection: 2 x 77 rows (row tail inside the second tile)
+    (3600, 1280, 5120),        # 3840^2 n=4 level-2 FF2: ragged rows (3600 = 28 * 128 + 16), long K
     (300, 1288, 192),          # N % 8 == 0 only
 ])
 @pytest.mark.parametrize("epi", ["plain", "bias", "bias_res"])
@@ -77,7 +77,7 @@ def test_linear_geglu_fused(M, K, D):
 
 
 def test_linear_repeated_launches_reuse_barriers():
-    """Persistent pairs, TMEM double buffering and the smem ring across many tiles and back-to-back launches."""
+    """Persistent CTAs and the smem ring (barrier phases) across many tiles and back-to-back launches."""
     from distrifuser_b200 import ops
     torch.manual_seed(23)
     x = torch.randn(4096, 640, device="cuda").half()

@@ -1,4 +1,4 @@
-"""End-to-end parity of the product path (fp16, sm_100a kernels, peer-memory comm) against golden vectors produced by
+"""End-to-end parity of the product path (fp16, sm_90a kernels, peer-memory comm) against golden vectors produced by
 the UNMODIFIED reference (fp32 CPU, gloo) on the same seeded tiny-SDXL UNet and inputs.
 
 Tolerance (stated per SURVEY 7 'fp16 statistics'): the reference side is fp32, the product computes in fp16 with
@@ -74,7 +74,7 @@ def test_unet_sd15_eight_gpus(golden_dir):
 
 def test_full_size_sdxl_unet_step_vs_oracle():
     """BASELINE configs[0]: the FULL SDXL UNet (2.57 B parameters, random init), 512x512, one CFG step, world_size 1 --
-    the fp16 sm_100a product path against the fp32 CPU oracle on the same weights and inputs.  Tolerance: the same
+    the fp16 sm_90a product path against the fp32 CPU oracle on the same weights and inputs.  Tolerance: the same
     relative bar as the tiny-UNet goldens (mean |err| < 1.2 % and max |err| < 12 % of the output's std; PSNR > 45 dB)."""
     import dataclasses
     from oracle import harness

@@ -1,7 +1,7 @@
 """Micro-benchmark of df_attn_fwd (fmha_fwd_kernel) at the SDXL self-attention shapes.  Default: a CUDA graph of `--launches`
 back-to-back launches on ROTATING q / kv / out buffers (total footprint > L2), timed with CUDA events over 5 replays -- the
 kernel's average duration as it runs inside the captured UNet step, without the host launch gaps that an eager
-event-bracketed launch picks up for 20-us kernels.  `--eager` times single launches (L2 flushed) like round 1 did;
+event-bracketed launch picks up for 20-us kernels.  `--eager` times single launches (L2 flushed);
 `--profile` brackets a single launch with cudaProfilerStart/Stop for ncu."""
 import argparse
 import ctypes as C

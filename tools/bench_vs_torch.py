@@ -2,7 +2,7 @@
   * attention: df_attn_fwd vs torch F.scaled_dot_product_attention (what the reference calls, attn.py:153) on the same tensors;
   * GroupNorm: df_groupnorm_fwd vs the reference module's eager op sequence (groupnorm.py:38-41,58-72: two means, stack, var,
     normalise, affine) and vs torch.nn.functional.group_norm.
-Informational (profiles/r1_vs_torch.txt); never a bench value."""
+Informational; never a bench value."""
 import ctypes as C
 import os
 import sys

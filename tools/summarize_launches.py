@@ -7,12 +7,12 @@ from collections import defaultdict
 
 def family(name: str) -> str:
     n = name
-    for pat, fam in ((r"fmha_fwd_kernel", "OURS fmha_fwd_kernel (tcgen05)"), (r"gn_fused_kernel", "OURS gn_fused_kernel"), (r"gn_stats_kernel", "OURS gn_stats_kernel"),
+    for pat, fam in ((r"fmha_fwd_kernel", "OURS fmha_fwd_kernel (wgmma)"), (r"gn_fused_kernel", "OURS gn_fused_kernel"), (r"gn_stats_kernel", "OURS gn_stats_kernel"),
                      (r"gn_apply_kernel", "OURS gn_apply_kernel"), (r"gn_exchange_kernel", "OURS gn_exchange_kernel"),
                      (r"halo_|publish_kernel|wait_kernel|step_begin|out_scatter|out_collect", "OURS comm/halo kernels"),
                      (r"geglu_kernel", "OURS geglu_kernel"), (r"add_layernorm_kernel", "OURS add_layernorm_kernel"),
                      (r"bias_residual_add_kernel", "OURS bias_residual_add_kernel (conv bias + residual)"),
-                     (r"linear_kernel|gemm_kernel", "OURS tcgen05 GEMM (df_linear)"),
+                     (r"linear_kernel|gemm_kernel", "OURS wgmma GEMM (df_linear)"),
                      # cuDNN's sm100 convs are "cutlass3x_sm100 ... fprop / implicit gemm" kernels: match them BEFORE the GEMM row
                      (r"cudnn|conv|implicit|fprop|wgrad|dgrad|nhwc|nchw", "library conv (cuDNN)"),
                      (r"nvjet|cutlass.*gemm|sm\d+_xmma_gemm|cublas|gemm|gemv", "library GEMM (cuBLAS)"),
