@@ -191,7 +191,7 @@ fmha_fwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
           if (seg != own_seg) {
             const int r = segs.rank[seg];
             if ((t == 0 || j == 0) && wait_flags) {
-              spin_until(comm.flags[comm.rank] + (size_t)idx * comm.world + r, rd, comm.spin_timeout_ns);
+              spin_until(flag_ptr(comm, comm.rank, idx, r), rd, comm.spin_timeout_ns);
               // the acquire above is a generic-proxy read; the peers' rows are fetched next through the async proxy (TMA)
               asm volatile("fence.proxy.async.global;" ::: "memory");
             }
@@ -402,25 +402,9 @@ fmha_fwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
 
 
 // ----------------------------------------------------------------------------------------- host side
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                  const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-EncodeTiledFn get_encode() {
-  static EncodeTiledFn fn = nullptr;
-  if (!fn) {
-    void* p = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess &&
-        q == cudaDriverEntryPointSuccess)
-      fn = (EncodeTiledFn)p;
-  }
-  return fn;
-}
-
 // 4-D view [d, nheads, rows, batch] of a row-major [batch, rows, pitch] fp16 matrix; box = [64, 1, 128, 1], 128B swizzle.
 int make_map(CUtensorMap* m, const void* base, int d, int nheads, int rows, int batch, int64_t pitch) {
-  EncodeTiledFn enc = get_encode();
+  EncodeTiledFn enc = tensor_map_encoder();
   DF_REQUIRE(enc != nullptr, "cuTensorMapEncodeTiled is not available from this driver");
   cuuint64_t dims[4] = {(cuuint64_t)d, (cuuint64_t)nheads, (cuuint64_t)rows, (cuuint64_t)batch};
   cuuint64_t strides[3] = {(cuuint64_t)d * 2, (cuuint64_t)pitch * 2, (cuuint64_t)rows * pitch * 2};
@@ -446,7 +430,7 @@ extern "C" int df_attn_make_kvmaps(df_comm_t comm, uint64_t tensor_off, uint64_t
   const int64_t pitch = 2 * (int64_t)heads * d;
   for (int k = 0; k < DF_NBANKS; ++k)
     for (int s = 0; s < comm.world; ++s) {
-      const char* base = (const char*)comm.base[comm.rank] + (uint64_t)k * comm.bank_stride + tensor_off + (uint64_t)s * slot_bytes;
+      const char* base = slot_ptr(comm, comm.rank, (uint32_t)k, tensor_off, slot_bytes, s);
       if (int rc = make_map(&host[k * comm.world + s], base, d, 2 * heads, lseg, b, pitch)) return rc;
     }
   DF_CHECK_CUDA(cudaMemcpyAsync(maps_out, host, sizeof(CUtensorMap) * DF_NBANKS * comm.world, cudaMemcpyHostToDevice,
@@ -456,16 +440,6 @@ extern "C" int df_attn_make_kvmaps(df_comm_t comm, uint64_t tensor_off, uint64_t
 }
 
 namespace {
-int sm_count() {
-  static int sms = 0;
-  if (!sms) {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    if (sms <= 0) sms = kSmCount;
-  }
-  return sms;
-}
 #ifndef DF_MIN_PART_TILES
 #define DF_MIN_PART_TILES 8    // a part of a split unit keeps at least this many K/V tiles (Q load + partial write + merge per part)
 #endif

@@ -38,6 +38,24 @@ extern "C" int df_device_sm_count(int* out) {
   return 0;
 }
 
+int df::sm_count() {
+  static int sms = 0;
+  if (!sms && (df_device_sm_count(&sms) != 0 || sms <= 0)) sms = kSmCount;
+  return sms;
+}
+
+EncodeTiledFn df::tensor_map_encoder() {
+  static EncodeTiledFn fn = nullptr;
+  if (!fn) {
+    void* p = nullptr;
+    cudaDriverEntryPointQueryResult q;
+    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess &&
+        q == cudaDriverEntryPointSuccess)
+      fn = (EncodeTiledFn)p;
+  }
+  return fn;
+}
+
 // ------------------------------------------------------------------------------------ symmetric memory
 extern "C" int df_symm_alloc(size_t bytes, void** dptr, void* ipc_handle_out_host) {
   DF_REQUIRE(dptr != nullptr && bytes > 0, "df_symm_alloc: bad arguments");
@@ -94,20 +112,6 @@ extern "C" int df_step_begin(uint32_t* clock, int kind, void* stream) {
 
 // ------------------------------------------------------------------------------------ publication
 // One load, `npeer` stores per 16-byte vector; the last CTA to finish stamps the peers' flags.
-__device__ __forceinline__ void signal_when_last(const df_comm_t& c, int idx, uint32_t peer_mask, uint32_t epoch) {
-  __threadfence_system();
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    uint32_t ticket = atomicAdd(&c.tickets[idx], 1u);
-    if (ticket == gridDim.x - 1) {
-      __threadfence();
-      c.tickets[idx] = 0;  // next launch on this tensor is stream-ordered after this kernel
-      for (int p = 0; p < c.world; ++p)
-        if (peer_mask >> p & 1) st_release_sys(c.flags[p] + (size_t)idx * c.world + c.rank, epoch);
-    }
-  }
-}
-
 // 128 threads, DF_PUB_UNROLL 16-byte loads in flight per thread: the transfer is bound by how many loads are outstanding (local
 // read latency ~1 us; the peer stores are posted).  What is exposed is the tail of the step's last publications, so a faster
 // transfer wins over taking fewer SM slots.
@@ -120,7 +124,7 @@ __global__ void __launch_bounds__(128, 8) publish_kernel(df_comm_t c, const char
   const uint32_t epoch = c.clock[0];
   const uint64_t total = rows * vec_per_row;
   const uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
-  const uint64_t bank_off = (uint64_t)(epoch % DF_NBANKS) * c.bank_stride + tensor_off + (uint64_t)c.rank * slot_bytes;
+  const uint64_t slot_off = slot_offset(c, epoch, tensor_off, slot_bytes, c.rank);
   constexpr int U = DF_PUB_UNROLL;
   uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
   for (; i + (U - 1) * stride < total; i += U * stride) {
@@ -134,7 +138,7 @@ __global__ void __launch_bounds__(128, 8) publish_kernel(df_comm_t c, const char
     }
     for (int p = 0; p < c.world; ++p) {
       if (!(peer_mask >> p & 1)) continue;
-      char* dst = (char*)c.base[p] + bank_off;
+      char* dst = (char*)c.base[p] + slot_off;
 #pragma unroll
       for (int u = 0; u < U; ++u) st_v4(dst + (i + u * stride) * 16, v[u]);
     }
@@ -144,9 +148,9 @@ __global__ void __launch_bounds__(128, 8) publish_kernel(df_comm_t c, const char
     if (rows > 1) { const uint32_t r = (uint32_t)i / (uint32_t)vec_per_row; soff = (uint64_t)r * src_pitch + (uint64_t)((uint32_t)i - r * (uint32_t)vec_per_row) * 16; }
     int4 v = ld_nc_v4(src + soff);
     for (int p = 0; p < c.world; ++p)
-      if (peer_mask >> p & 1) st_v4((char*)c.base[p] + bank_off + i * 16, v);
+      if (peer_mask >> p & 1) st_v4((char*)c.base[p] + slot_off + i * 16, v);
   }
-  signal_when_last(c, idx, peer_mask, epoch);
+  signal_when_last(c, &c.tickets[idx], gridDim.x, idx, peer_mask, epoch);
 }
 
 extern "C" int df_slot_publish(df_comm_t comm, const void* src, uint64_t rows, uint64_t row_bytes, uint64_t src_pitch,
@@ -167,11 +171,7 @@ extern "C" int df_slot_publish(df_comm_t comm, const void* src, uint64_t rows, u
   return 0;
 }
 
-__global__ void wait_kernel(df_comm_t c, int idx, uint32_t src_mask) {
-  const uint32_t want = c.clock[1];
-  int s = threadIdx.x;
-  if (s < c.world && (src_mask >> s & 1)) spin_until(c.flags[c.rank] + (size_t)idx * c.world + s, want, c.spin_timeout_ns);
-}
+__global__ void wait_kernel(df_comm_t c, int idx, uint32_t src_mask) { wait_sources(c, idx, src_mask, c.clock[1]); }
 extern "C" int df_slot_wait(df_comm_t comm, int idx, uint32_t src_mask, void* stream) {
   if (src_mask == 0) return 0;
   wait_kernel<<<1, 32, 0, (cudaStream_t)stream>>>(comm, idx, src_mask);
@@ -199,15 +199,14 @@ __global__ void __launch_bounds__(256) out_scatter_kernel(df_comm_t c, const V* 
       *d = v;
     }
   }
-  signal_when_last(c, idx, world_mask, epoch);
+  signal_when_last(c, &c.tickets[idx], gridDim.x, idx, world_mask, epoch);
 }
 
 template <typename V>
 __global__ void __launch_bounds__(256) out_collect_kernel(df_comm_t c, V* __restrict__ out, int64_t total_vec, int idx,
                                                           uint64_t tensor_off) {
   const uint32_t epoch = c.clock[2];
-  if (threadIdx.x < c.world) spin_until(c.flags[c.rank] + (size_t)idx * c.world + threadIdx.x, epoch, c.spin_timeout_ns);
-  __syncthreads();
+  wait_sources(c, idx, 0xffffffffu, epoch);
   const V* src = (const V*)slot_ptr(c, c.rank, epoch, tensor_off, 0, 0);
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total_vec; i += (int64_t)gridDim.x * blockDim.x)
     out[i] = src[i];

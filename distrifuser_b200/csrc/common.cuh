@@ -1,5 +1,6 @@
 // distrifuser_b200 -- shared device/host helpers (sm_90a only).
 #pragma once
+#include <cuda.h>
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -11,6 +12,14 @@ namespace df {
 
 // SMs of the H100 SXM the grid-size heuristics are tuned for (kernels that size a persistent grid query the device)
 constexpr int kSmCount = 132;
+// SMs of the current device, queried once (kSmCount if the query fails)
+int sm_count();
+
+typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
+                                  const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
+                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+// cuTensorMapEncodeTiled of the driver, looked up once (nullptr if the driver does not provide it)
+EncodeTiledFn tensor_map_encoder();
 
 void set_error(const char* fmt, ...);
 
@@ -115,9 +124,57 @@ inline cudaError_t launch_pdl(unsigned family, void (*kernel)(KArgs...), dim3 gr
   return cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
 }
 
-__device__ __forceinline__ char* slot_ptr(const df_comm_t& c, int rank, uint32_t epoch, uint64_t tensor_off,
-                                          uint64_t slot_bytes, int src) {
-  return (char*)c.base[rank] + (uint64_t)(epoch % DF_NBANKS) * c.bank_stride + tensor_off + (uint64_t)src * slot_bytes;
+// ------------------------------------------------------------------ cross-rank protocol (include/distrifuser_b200.h: arena layout)
+// A writer stores into slot(epoch, idx, src = its rank) of the readers' arenas, then stamps flags[idx*world + src] = epoch on
+// each reader (release, system scope); a reader acquires that flag before it reads the slot.
+
+// byte offset of slot(epoch, tensor, src) in every member's arena
+__host__ __device__ __forceinline__ uint64_t slot_offset(const df_comm_t& c, uint32_t epoch, uint64_t tensor_off,
+                                                         uint64_t slot_bytes, int src) {
+  return (uint64_t)(epoch % DF_NBANKS) * c.bank_stride + tensor_off + (uint64_t)src * slot_bytes;
+}
+__host__ __device__ __forceinline__ char* slot_ptr(const df_comm_t& c, int rank, uint32_t epoch, uint64_t tensor_off,
+                                                   uint64_t slot_bytes, int src) {
+  return (char*)c.base[rank] + slot_offset(c, epoch, tensor_off, slot_bytes, src);
+}
+
+// flag word of tensor `idx` and source `src` in the flag array of `member`
+__device__ __forceinline__ uint32_t* flag_ptr(const df_comm_t& c, int member, int idx, int src) {
+  return c.flags[member] + (size_t)idx * c.world + src;
+}
+
+// stamps this rank's flag of tensor `idx` with `epoch` at the members in `mask` (the caller has fenced its slot stores); a CTA
+// may share the members out: the calling thread takes members first, first + step, ...
+__device__ __forceinline__ void stamp_flags(const df_comm_t& c, int idx, uint32_t mask, uint32_t epoch, int first = 0, int step = 1) {
+  for (int p = first; p < c.world; p += step)
+    if (mask >> p & 1) st_release_sys(flag_ptr(c, p, idx, c.rank), epoch);
+}
+
+// the CTA waits until this rank's flags of tensor `idx` from every source in `mask` reached `epoch` (thread s waits on source s)
+__device__ __forceinline__ void wait_sources(const df_comm_t& c, int idx, uint32_t mask, uint32_t epoch) {
+  const int s = threadIdx.x;
+  if (s < c.world && (mask >> s & 1)) spin_until(flag_ptr(c, c.rank, idx, s), epoch, c.spin_timeout_ns);
+  __syncthreads();
+}
+
+// member mask of the patch neighbours of a halo exchange (-1: image border)
+__device__ __forceinline__ uint32_t neighbour_mask(int up, int down) {
+  return (up >= 0 ? 1u << up : 0u) | (down >= 0 ? 1u << down : 0u);
+}
+
+// Called by every thread of each of the `nctas` CTAs of a grid after its slot stores: the last CTA to take a ticket resets the
+// counter (the next launch that uses it is stream-ordered after this one) and stamps the flags of `mask`.
+__device__ __forceinline__ void signal_when_last(const df_comm_t& c, unsigned int* ticket, unsigned int nctas, int idx,
+                                                 uint32_t mask, uint32_t epoch) {
+  __threadfence_system();
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    if (atomicAdd(ticket, 1u) == nctas - 1) {
+      __threadfence();
+      *ticket = 0;
+      stamp_flags(c, idx, mask, epoch);
+    }
+  }
 }
 
 }  // namespace df

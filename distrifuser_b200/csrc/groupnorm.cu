@@ -1,11 +1,9 @@
 // distrifuser_b200 -- GroupNorm with cross-rank sufficient statistics (NHWC fp16).
 // Replaces DistriGroupNorm.forward (distrifuser/modules/pp/groupnorm.py:14-97): the ~10 eager reduction /
-// elementwise kernels and the 256-byte NCCL all_gather / all_reduce per layer become
-//   (1) gn_stats_kernel    one HBM read, fp32 per-channel register accumulation, per-CTA partial moments; the LAST CTA to
-//                          finish reduces the partials, exchanges (E[x], E[x^2]) with the patch group through peer stores +
-//                          release/acquire flags over NVLink and applies the mode formula (gn_exchange)
-//   (2) gn_apply_kernel    one read (L2-resident for <= ~60 MB activations) + one write, optional fused SiLU
-// Both accept a per-(sample, channel) addend so that ResnetBlock2D's `conv1(x) + time_emb` never materialises.
+// elementwise kernels and the 256-byte NCCL all_gather / all_reduce per layer become ONE launch (gn_fused_kernel): one HBM
+// read with fp32 per-channel register accumulation, a grid barrier, the exchange of (E[x], E[x^2]) with the patch group through
+// peer stores + release/acquire flags over NVLink, and the normalisation with optional fused SiLU.  It accepts a
+// per-(sample, channel) addend so that ResnetBlock2D's `conv1(x) + time_emb` never materialises.
 #include <string.h>
 
 #include "common.cuh"
@@ -30,6 +28,10 @@ struct GnPlan {
   int ppc;      // pixels per CTA
 };
 
+constexpr int kGnMaxSmem = 32 * 1024;   // dynamic shared memory of gn_fused_kernel: lanes * C <= 4096 moments
+
+int gn_resident_ctas();
+
 inline GnPlan gn_plan(int b, int h, int w, int C) {
   GnPlan p;
   p.V = C / 8;
@@ -41,9 +43,11 @@ inline GnPlan gn_plan(int b, int h, int w, int C) {
   int want = (2 * kSmCount + b - 1) / b;                  // ~2 CTAs per SM over the batch
   int cap = hw / (p.lanes * 8);                      // >= 8 pixels per thread
   if (cap < 1) cap = 1;
-  p.nchunk = want < cap ? want : cap;
-  p.ppc = (hw + p.nchunk - 1) / p.nchunk;
-  p.nchunk = (hw + p.ppc - 1) / p.ppc;
+  auto split = [&](int n) { p.ppc = (hw + n - 1) / n; p.nchunk = (hw + p.ppc - 1) / p.ppc; };
+  split(want < cap ? want : cap);
+  // the grid barrier needs every CTA resident at once: fewer, longer chunks where the batch would not fit
+  const int resident = gn_resident_ctas();
+  if (p.nchunk * b > resident && resident >= b) split(resident / b);
   return p;
 }
 
@@ -57,9 +61,8 @@ __device__ __forceinline__ void unpack8(const int4& v, float* f) {
   }
 }
 
-struct GnExchange {   // everything the last CTA needs to finish the statistics (was a separate 1-CTA kernel: 23 us of latency)
+struct GnExchange {   // grid barrier and cross-rank exchange of the statistics
   df_comm_t c;
-  float2* coef;
   unsigned int* ticket;
   int bG, nchunk_total;
   float inv_ne, bessel, eps;
@@ -84,15 +87,11 @@ struct GnHalo {
   df_comm_t c;
 };
 
-__device__ void gn_exchange(const GnExchange& e, const float2* __restrict__ partial, int G, int nchunk, float2* mine);
-
-// Statistics pass of one CTA; returns true in the LAST CTA of the grid after it has run the exchange and written coef[].
-// STREAM = true: loads bypass L1 (two-kernel path: the data is touched once); false: default caching, so that the apply pass
-// of the fused kernel finds this CTA's pixels in L1 / L2.
-template <bool STREAM>
-__device__ __forceinline__ bool gn_stats_body(const __half* __restrict__ x, const __half* __restrict__ addend, int64_t addend_pitch,
-                                              float2* __restrict__ partial, int hw, int C, int G, int V, int lanes,
-                                              int ppc, const GnExchange& ex, float2* ch, bool partials_only = false) {
+// Statistics pass of one CTA: the group moments of its pixels -> partial[].  Loads use the default caching, so that the
+// normalise pass finds this CTA's pixels in L1 / L2.
+__device__ __forceinline__ void gn_moments(const __half* __restrict__ x, const __half* __restrict__ addend, int64_t addend_pitch,
+                                           float2* __restrict__ partial, int hw, int C, int G, int V, int lanes,
+                                           int ppc, float2* ch) {
   const int b = blockIdx.y, chunk = blockIdx.x, nchunk = gridDim.x;
   const int tid = threadIdx.x;
   const int v = tid % V, pl = tid / V;
@@ -108,7 +107,7 @@ __device__ __forceinline__ bool gn_stats_body(const __half* __restrict__ x, cons
     for (; p + (U - 1) * lanes < p1; p += U * lanes) {
       int4 r[U];
 #pragma unroll
-      for (int u = 0; u < U; ++u) r[u] = STREAM ? ld_nc_v4(base + (size_t)(p + u * lanes) * C) : ld_v4(base + (size_t)(p + u * lanes) * C);
+      for (int u = 0; u < U; ++u) r[u] = ld_v4(base + (size_t)(p + u * lanes) * C);
 #pragma unroll
       for (int u = 0; u < U; ++u) {
         float f[8];
@@ -119,7 +118,7 @@ __device__ __forceinline__ bool gn_stats_body(const __half* __restrict__ x, cons
     }
     for (; p < p1; p += lanes) {
       float f[8];
-      unpack8(STREAM ? ld_nc_v4(base + (size_t)p * C) : ld_v4(base + (size_t)p * C), f);
+      unpack8(ld_v4(base + (size_t)p * C), f);
 #pragma unroll
       for (int j = 0; j < 8; ++j) { float t = f[j] + ad[j]; s[j] += t; ss[j] = fmaf(t, t, ss[j]); }
     }
@@ -149,108 +148,9 @@ __device__ __forceinline__ bool gn_stats_body(const __half* __restrict__ x, cons
     for (int part = 0; part < parts; ++part) { a += fold[part * G + g].x; q += fold[part * G + g].y; }
     partial[((size_t)b * nchunk + chunk) * G + g] = make_float2(a, q);
   }
-  if (partials_only) return false;                // fused kernel: grid barrier + per-CTA reduction follow (gn_fused_kernel)
-  // last CTA of the grid finishes the job: reduce the partials, exchange with the patch group, write (mean, rstd)
-  __shared__ bool is_last;
-  __threadfence();
-  __syncthreads();
-  if (tid == 0) {
-    unsigned int t = atomicAdd(ex.ticket, 1u);
-    is_last = (t == (unsigned int)ex.nchunk_total - 1);
-    if (is_last) *ex.ticket = 0;
-  }
-  __syncthreads();
-  if (!is_last) return false;
-  __threadfence();
-  gn_exchange(ex, partial, G, nchunk, ch);
-  return true;
 }
 
-__global__ void __launch_bounds__(512) gn_stats_kernel(const __half* __restrict__ x, const __half* __restrict__ addend, int64_t addend_pitch,
-                                                       float2* __restrict__ partial, int hw, int C, int G, int V, int lanes,
-                                                       int ppc, GnExchange ex) {
-  extern __shared__ float2 ch[];  // [lanes][C] per-channel (sum, sum of squares); reused as float2 mine[bG] by the last CTA
-  gn_stats_body<true>(x, addend, addend_pitch, partial, hw, C, G, V, lanes, ppc, ex, ch);
-}
-
-// mode: 0 local, 1 synchronous exchange, 2 corrected_async_gn, 3 stale_gn   (see include/distrifuser_b200.h)
-__device__ void gn_exchange(const GnExchange& e, const float2* __restrict__ partial, int G, int nchunk, float2* mine) {
-  const df_comm_t& c = e.c;
-  float2* __restrict__ coef = e.coef;
-  const int bG = e.bG, mode = e.mode, neg_fb = e.neg_fb, idx = e.idx;
-  const float inv_ne = e.inv_ne, bessel = e.bessel, eps = e.eps;
-  const uint64_t tensor_off = e.tensor_off, slot_bytes = e.slot_bytes;
-  const uint32_t group_mask = e.group_mask;
-  const int tid = threadIdx.x, nthr = blockDim.x;
-  // parallel reduction of the per-CTA partials: `tpp` threads per (sample, group) pair, then a shared-memory fold
-  __shared__ float2 red[512];
-  const int tpp = max(1, min(nthr / bG, 8));      // bG * tpp <= 512 (host guard: bG <= 512)
-  for (int e = tid; e < bG * tpp; e += nthr) {    // stride loop: bG may exceed the block (b*groups = 512 on 320 threads)
-    const int i = e / tpp, r = e - i * tpp;
-    const int b = i / G, g = i - b * G;
-    float s = 0.f, ss = 0.f;
-    for (int k = r; k < nchunk; k += tpp) {
-      float2 p = partial[((size_t)b * nchunk + k) * G + g];
-      s += p.x; ss += p.y;
-    }
-    red[e] = make_float2(s, ss);
-  }
-  __syncthreads();
-  for (int i = tid; i < bG; i += nthr) {
-    float s = 0.f, ss = 0.f;
-    for (int r = 0; r < tpp; ++r) { s += red[i * tpp + r].x; ss += red[i * tpp + r].y; }
-    mine[i] = make_float2(s * inv_ne, ss * inv_ne);
-  }
-  __syncthreads();
-  const int n = __popc(group_mask);
-  uint32_t pub = 0, rd = 0;
-  if (mode != 0) { pub = c.clock[0]; rd = c.clock[1]; }
-  if (mode == 1) rd = pub;  // a synchronous exchange reads THIS epoch even inside an asynchronous step (sync_gn, groupnorm.py:74-80)
-
-  auto publish = [&]() {
-    for (int p = 0; p < c.world; ++p) {
-      if (!(group_mask >> p & 1)) continue;
-      float2* dst = (float2*)slot_ptr(c, p, pub, tensor_off, slot_bytes, c.rank);
-      for (int i = tid; i < bG; i += nthr) dst[i] = mine[i];
-    }
-    __threadfence_system();
-    __syncthreads();
-    if (tid < c.world && (group_mask >> tid & 1)) st_release_sys(c.flags[tid] + (size_t)idx * c.world + c.rank, pub);
-  };
-  auto wait_all = [&]() {
-    if (tid < c.world && (group_mask >> tid & 1)) spin_until(c.flags[c.rank] + (size_t)idx * c.world + tid, rd, c.spin_timeout_ns);
-    __syncthreads();
-  };
-
-  if (mode == 1) publish();          // fresh statistics are needed by everyone in this very step
-  if (mode != 0) wait_all();         // sync: this epoch's; async: the previous epoch's (1-step stale)
-
-  for (int i = tid; i < bG; i += nthr) {
-    float2 m = mine[i];
-    float mean = m.x, msq = m.y;
-    if (mode != 0) {
-      float sx = 0.f, sy = 0.f;
-      float2 own_stale = make_float2(0.f, 0.f);
-      for (int p = 0; p < c.world; ++p) {
-        if (!(group_mask >> p & 1)) continue;
-        float2 v = ((const float2*)slot_ptr(c, c.rank, rd, tensor_off, slot_bytes, p))[i];
-        if (p == c.rank) own_stale = v;
-        sx += v.x; sy += v.y;
-      }
-      const float invn = 1.f / (float)n;
-      if (mode == 1) { mean = sx * invn; msq = sy * invn; }                                     // groupnorm.py:47,80
-      else if (mode == 2) { mean = sx * invn + (m.x - own_stale.x); msq = sy * invn + (m.y - own_stale.y); }  // :49-51
-      else { mean = (sx - own_stale.x + m.x) * invn; msq = (sy - own_stale.y + m.y) * invn; }  // :52-55
-    }
-    float var = msq - mean * mean;
-    if (neg_fb && var < 0.f) var = m.y - m.x * m.x;                                             // :60-63
-    var *= bessel;                                                                              // :65-66
-    coef[i] = make_float2(mean, rsqrtf(var + eps));
-  }
-  if (mode >= 2) { __syncthreads(); publish(); }   // asynchronous: ship this step's statistics for the next step
-}
-
-// ---- fused kernel: statistics finished by EVERY CTA for its own sample (no serial exchange in one CTA, no coef[] round trip)
+// ---- after the grid barrier EVERY CTA finishes the statistics of its own sample
 __device__ __forceinline__ float2 ld_cg_f2(const float2* p) {      // L2 load: the partials were written during this launch
   float2 r;
   asm volatile("ld.global.cg.v2.f32 {%0, %1}, [%2];" : "=f"(r.x), "=f"(r.y) : "l"(p) : "memory");
@@ -302,19 +202,18 @@ __device__ void gn_publish_all(const GnExchange& e, const float2* __restrict__ p
   }
   __threadfence_system();
   __syncthreads();
-  if (tid < c.world && (e.group_mask >> tid & 1)) st_release_sys(c.flags[tid] + (size_t)e.idx * c.world + c.rank, pub);
+  stamp_flags(c, e.idx, e.group_mask, pub, tid, nthr);
 }
 
 // (mean, rstd) of the G groups of sample b from this rank's statistics `mine` and, in the exchange modes, the patch group's
-// slots of the read epoch (groupnorm.py:40-66; same arithmetic and order as gn_exchange).
+// slots of the read epoch (groupnorm.py:40-66).
 __device__ __forceinline__ void gn_coef_sample(const GnExchange& e, int b, int G, const float2* mine, float2* coef_s) {
   const df_comm_t& c = e.c;
   const int tid = threadIdx.x, nthr = blockDim.x, mode = e.mode;
   uint32_t rd = 0;
   if (mode != 0) {
     rd = mode == 1 ? c.clock[0] : c.clock[1];   // a synchronous exchange reads THIS epoch even inside an asynchronous step
-    if (tid < c.world && (e.group_mask >> tid & 1)) spin_until(c.flags[c.rank] + (size_t)e.idx * c.world + tid, rd, c.spin_timeout_ns);
-    __syncthreads();
+    wait_sources(c, e.idx, e.group_mask, rd);
   }
   const int n = __popc(e.group_mask);
   for (int g = tid; g < G; g += nthr) {
@@ -342,12 +241,11 @@ __device__ __forceinline__ void gn_coef_sample(const GnExchange& e, int b, int G
   __syncthreads();
 }
 
-template <bool STREAM>
-__device__ __forceinline__ void gn_apply_body(const __half* __restrict__ x, const __half* __restrict__ addend, int64_t addend_pitch,
-                                              __half* __restrict__ y, const __half* __restrict__ gamma,
-                                              const __half* __restrict__ beta,
-                                              const float2* __restrict__ coef, int hw, int C, int G, int V, int lanes,
-                                              int ppc, int silu, const GnHalo& halo) {
+__device__ __forceinline__ void gn_normalise(const __half* __restrict__ x, const __half* __restrict__ addend, int64_t addend_pitch,
+                                             __half* __restrict__ y, const __half* __restrict__ gamma,
+                                             const __half* __restrict__ beta,
+                                             const float2* coef, int hw, int C, int G, int V, int lanes,
+                                             int ppc, int silu, const GnHalo& halo) {
   const int b = blockIdx.y, chunk = blockIdx.x;
   const int tid = threadIdx.x;
   const int v = tid % V, pl = tid / V;
@@ -360,8 +258,7 @@ __device__ __forceinline__ void gn_apply_body(const __half* __restrict__ x, cons
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
       int ch = v * 8 + j;
-      float2 mr;                       // generic load: coef[] is shared memory in the fused kernel, global otherwise
-      asm volatile("ld.v2.f32 {%0, %1}, [%2];" : "=f"(mr.x), "=f"(mr.y) : "l"(coef + b * G + ch / cpg) : "memory");
+      const float2 mr = coef[ch / cpg];
       float ga = gamma ? __half2float(gamma[ch]) : 1.f, be = beta ? __half2float(beta[ch]) : 0.f;
       sc[j] = mr.y * ga;
       sh[j] = be - mr.x * sc[j];
@@ -409,27 +306,15 @@ __device__ __forceinline__ void gn_apply_body(const __half* __restrict__ x, cons
     for (; p + 3 * lanes < p1; p += 4 * lanes) {
       int4 r[4];
 #pragma unroll
-      for (int u = 0; u < 4; ++u) r[u] = STREAM ? ld_nc_v4(x + base + (size_t)(p + u * lanes) * C) : ld_v4(x + base + (size_t)(p + u * lanes) * C);
+      for (int u = 0; u < 4; ++u) r[u] = ld_v4(x + base + (size_t)(p + u * lanes) * C);
 #pragma unroll
       for (int u = 0; u < 4; ++u) emit(p + u * lanes, xform(r[u]));
     }
-    for (; p < p1; p += lanes) emit(p, xform(STREAM ? ld_nc_v4(x + base + (size_t)p * C) : ld_v4(x + base + (size_t)p * C)));
+    for (; p < p1; p += lanes) emit(p, xform(ld_v4(x + base + (size_t)p * C)));
   }
   if (!halo.enabled) return;
-  // ---- boundary rows shipped: the last CTA of the grid stamps the neighbours' flags (protocol of halo_push_kernel)
-  if (halo.push) {
-    __threadfence_system();
-    __syncthreads();
-    if (tid == 0) {
-      const unsigned int tk = atomicAdd(halo.ticket2, 1u);
-      if (tk == gridDim.x * gridDim.y - 1) {
-        __threadfence();
-        *halo.ticket2 = 0;
-        if (halo.up >= 0) st_release_sys(halo.c.flags[halo.up] + (size_t)halo.idx * halo.c.world + halo.c.rank, pub);
-        if (halo.down >= 0) st_release_sys(halo.c.flags[halo.down] + (size_t)halo.idx * halo.c.world + halo.c.rank, pub);
-      }
-    }
-  }
+  // ---- boundary rows shipped: the last CTA of the grid stamps the neighbours' flags
+  if (halo.push) signal_when_last(halo.c, halo.ticket2, gridDim.x * gridDim.y, halo.idx, neighbour_mask(halo.up, halo.down), pub);
   // ---- margin rows of sample b: first chunk fills the top one, last chunk the bottom one (zeros at the image border)
   const bool top = chunk == 0, bottom = chunk == (int)gridDim.x - 1;
   if (!top && !bottom) return;
@@ -442,8 +327,7 @@ __device__ __forceinline__ void gn_apply_body(const __half* __restrict__ x, cons
     const int src = side == 0 ? halo.up : halo.down;
     __half* dst = y + ((size_t)b * (halo.h + 2) + (side == 0 ? 0 : halo.h + 1)) * row_el;
     if (src >= 0) {
-      if (halo.wait_flags && tid == 0) spin_until(halo.c.flags[halo.c.rank] + (size_t)halo.idx * halo.c.world + src, rd, halo.c.spin_timeout_ns);
-      __syncthreads();
+      if (halo.wait_flags) wait_sources(halo.c, halo.idx, 1u << src, rd);
       // top margin = the up neighbour's LAST row (its part 1); bottom margin = the down neighbour's FIRST row (part 0)
       const __half* from = (const __half*)slot_ptr(halo.c, halo.c.rank, rd, halo.off, halo.slot_bytes, src) +
                            ((side == 0 ? nb : 0) + b) * row_el;
@@ -453,14 +337,6 @@ __device__ __forceinline__ void gn_apply_body(const __half* __restrict__ x, cons
       for (int i = tid; i < row_vec; i += blockDim.x) st_v4(dst + (size_t)i * 8, zero);
     }
   }
-}
-
-__global__ void __launch_bounds__(512) gn_apply_kernel(const __half* __restrict__ x, const __half* __restrict__ addend, int64_t addend_pitch,
-                                                       __half* __restrict__ y, const __half* __restrict__ gamma,
-                                                       const __half* __restrict__ beta,
-                                                       const float2* __restrict__ coef, int hw, int C, int G, int V, int lanes,
-                                                       int ppc, int silu, GnHalo halo) {
-  gn_apply_body<true>(x, addend, addend_pitch, y, gamma, beta, coef, hw, C, G, V, lanes, ppc, silu, halo);
 }
 
 // ONE launch: partial moments -> grid barrier -> every CTA finishes the statistics of ITS sample -> normalise.  Every CTA of the
@@ -484,7 +360,7 @@ __global__ void __launch_bounds__(512, 2) gn_fused_kernel(const __half* __restri
   GN_TR(0, blockIdx.x == 0 && blockIdx.y == 0 && threadIdx.x == 0);
   if (threadIdx.x == 0) my_gen = ld_volatile_u32(gen);   // read before this CTA's ticket: the bump needs every CTA's ticket
   __syncthreads();
-  gn_stats_body<false>(x, addend, addend_pitch, partial, hw, C, G, V, lanes, ppc, ex, ch, true);
+  gn_moments(x, addend, addend_pitch, partial, hw, C, G, V, lanes, ppc, ch);
   // ---- grid barrier: ticket, the last arriver resets it and bumps the generation
   __threadfence();
   __syncthreads();
@@ -520,9 +396,23 @@ __global__ void __launch_bounds__(512, 2) gn_fused_kernel(const __half* __restri
     gn_publish_all(ex, partial, G, nchunk, red2, red2 + G * tpp);
   }
   GN_TR(5, blockIdx.x == 0 && blockIdx.y == 0 && threadIdx.x == 0);
-  gn_apply_body<false>(x, addend, addend_pitch, y, gamma, beta, coef_s - (size_t)b * G, hw, C, G, V, lanes, ppc, silu, halo);
+  gn_normalise(x, addend, addend_pitch, y, gamma, beta, coef_s, hw, C, G, V, lanes, ppc, silu, halo);
   GN_TR(6, blockIdx.x == 0 && blockIdx.y == 0 && threadIdx.x == 0);
   GN_TR(7, is_last && threadIdx.x == 0);
+}
+
+// CTAs of gn_fused_kernel the device holds at once (at its largest block and shared-memory size), queried once
+int gn_resident_ctas() {
+  static int n = -1;
+  if (n < 0) {
+    int per_sm = 0;
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, gn_fused_kernel, 512, kGnMaxSmem) != cudaSuccess) {
+      per_sm = 0;
+      cudaGetLastError();
+    }
+    n = per_sm * sm_count();
+  }
+  return n;
 }
 
 #ifdef DF_GN_TRACE
@@ -539,7 +429,7 @@ namespace {
 
 extern "C" size_t df_groupnorm_scratch_bytes(int b, int groups, int h, int w, int C) {
   GnPlan p = gn_plan(b, h, w, C);
-  return ((size_t)b * p.nchunk * groups + (size_t)b * groups) * sizeof(float2) + 256;
+  return (size_t)b * p.nchunk * groups * sizeof(float2) + 256;
 }
 
 namespace {
@@ -558,50 +448,32 @@ int groupnorm_impl(df_comm_t comm, const void* x, const void* addend, int64_t ad
              "df_groupnorm_fwd: statistics slot too small or rank outside its own group");
   cudaStream_t st = (cudaStream_t)stream;
   GnPlan p = gn_plan(b, h, w, C);
-  // scratch: [ticket (256 B, zero-initialised by the caller once)] [partials] [coef]
+  // scratch: [tickets (256 B, zero-initialised by the caller once)] [partials]
   unsigned int* ticket = (unsigned int*)scratch;
   halo.ticket2 = ticket + 2;
   float2* partial = (float2*)((char*)scratch + 256);
-  float2* coef = partial + (size_t)b * p.nchunk * groups;
   const int hw = h * w;
   const long long ne = (long long)(C / groups) * hw;
   GnExchange ex;
-  ex.c = comm; ex.coef = coef; ex.ticket = ticket; ex.bG = b * groups; ex.nchunk_total = p.nchunk * b;
+  ex.c = comm; ex.ticket = ticket; ex.bG = b * groups; ex.nchunk_total = p.nchunk * b;
   ex.inv_ne = (float)(1.0 / (double)ne);
   ex.bessel = bessel ? (float)((double)ne / (double)(ne - 1)) : 1.f;
   ex.eps = eps; ex.mode = mode; ex.neg_fb = neg_var_fallback; ex.idx = idx;
   ex.tensor_off = tensor_off; ex.slot_bytes = slot_bytes; ex.group_mask = group_mask;
-  size_t smem = (size_t)p.lanes * C * sizeof(float2);           // <= 32 KiB (lanes * C <= 4096)
-  if (smem < (size_t)b * groups * sizeof(float2)) smem = (size_t)b * groups * sizeof(float2);
-  {                                                             // fused kernel, after the fold: 2 x (red[G*tpp] + mine[G]) + coef[G]
+  size_t smem = (size_t)p.lanes * C * sizeof(float2);
+  {                                                             // after the fold: 2 x (red[G*tpp] + mine[G]) + coef[G]
     int tpp = p.threads / groups; if (tpp > 16) tpp = 16; if (tpp < 1) tpp = 1;
     const size_t need = (size_t)(2 * (groups * tpp + groups) + groups) * sizeof(float2);
     if (smem < need) smem = need;
   }
-  // one launch when the whole grid is resident at once (always, for the plans of gn_plan on an H100: <= 2 CTAs per SM)
-  static int fused_capacity = -1;
-  if (fused_capacity < 0) {
-    int dev = 0, sms = 0, per_sm = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, gn_fused_kernel, 512, 32 * 1024) != cudaSuccess) per_sm = 0;
-    fused_capacity = per_sm * sms;
-    cudaGetLastError();
-  }
-  if (p.nchunk * b <= fused_capacity && smem <= 32 * 1024) {
-    unsigned int* gen = ticket + 1;
-    DF_CHECK_CUDA(launch_pdl(PDL_GN, gn_fused_kernel, dim3(p.nchunk, b), dim3(p.threads), smem, st, (const __half*)x, (const __half*)addend, addend_pitch,
-                             (__half*)y, (const __half*)gamma, (const __half*)beta, partial, hw, C, groups, p.V,
-                             p.lanes, p.ppc, fuse_silu, ex, gen, halo));
-    return 0;
-  }
-  gn_stats_kernel<<<dim3(p.nchunk, b), p.threads, smem, st>>>((const __half*)x, (const __half*)addend, addend_pitch, partial, hw, C, groups,
-                                                             p.V, p.lanes, p.ppc, ex);
-  DF_CHECK_LAUNCH();
-  gn_apply_kernel<<<dim3(p.nchunk, b), p.threads, 0, st>>>((const __half*)x, (const __half*)addend, addend_pitch, (__half*)y,
-                                                           (const __half*)gamma, (const __half*)beta, coef, hw, C, groups, p.V,
-                                                           p.lanes, p.ppc, fuse_silu, halo);
-  DF_CHECK_LAUNCH();
+  // the grid barrier spins on CTAs that have not arrived: all of them must be resident at once
+  DF_REQUIRE(p.nchunk * b <= gn_resident_ctas(), "df_groupnorm_fwd: grid of %d CTAs exceeds the %d this device holds at once",
+             p.nchunk * b, gn_resident_ctas());
+  DF_REQUIRE(smem <= (size_t)kGnMaxSmem, "df_groupnorm_fwd: %zu bytes of shared memory exceed %d", smem, kGnMaxSmem);
+  unsigned int* gen = ticket + 1;
+  DF_CHECK_CUDA(launch_pdl(PDL_GN, gn_fused_kernel, dim3(p.nchunk, b), dim3(p.threads), smem, st, (const __half*)x, (const __half*)addend, addend_pitch,
+                           (__half*)y, (const __half*)gamma, (const __half*)beta, partial, hw, C, groups, p.V,
+                           p.lanes, p.ppc, fuse_silu, ex, gen, halo));
   return 0;
 }
 }  // namespace

@@ -29,32 +29,14 @@ __global__ void __launch_bounds__(256) halo_push_kernel(df_comm_t c, const char*
     uint64_t src_row = bb * h + (part == 0 ? 0 : h - 1);
     st_v4(dst + (bb * row_vec + q) * 16, ld_nc_v4(x + (src_row * row_vec + q) * 16));
   }
-  uint32_t mask = 0;
-  if (up_rank >= 0) mask |= 1u << up_rank;
-  if (down_rank >= 0) mask |= 1u << down_rank;
-  // inline copy of comm.cu's last-CTA signal (kept here so the kernel has no cross-TU device call)
-  __threadfence_system();
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    uint32_t ticket = atomicAdd(&c.tickets[idx], 1u);
-    if (ticket == gridDim.x - 1) {
-      __threadfence();
-      c.tickets[idx] = 0;
-      for (int p = 0; p < c.world; ++p)
-        if (mask >> p & 1) st_release_sys(c.flags[p] + (size_t)idx * c.world + c.rank, epoch);
-    }
-  }
+  signal_when_last(c, &c.tickets[idx], gridDim.x, idx, neighbour_mask(up_rank, down_rank), epoch);
 }
 
 __global__ void __launch_bounds__(256) halo_assemble_kernel(df_comm_t c, const char* __restrict__ x, char* __restrict__ xp,
                                                             int b, int h, uint64_t row_vec, int idx, uint64_t tensor_off,
                                                             uint64_t slot_bytes, int up_rank, int down_rank, int wait_flags) {
   const uint32_t rd = (up_rank >= 0 || down_rank >= 0) ? c.clock[1] : 0u;
-  if (wait_flags) {
-    if (threadIdx.x == 0 && up_rank >= 0) spin_until(c.flags[c.rank] + (size_t)idx * c.world + up_rank, rd, c.spin_timeout_ns);
-    if (threadIdx.x == 1 && down_rank >= 0) spin_until(c.flags[c.rank] + (size_t)idx * c.world + down_rank, rd, c.spin_timeout_ns);
-    __syncthreads();
-  }
+  if (wait_flags) wait_sources(c, idx, neighbour_mask(up_rank, down_rank), rd);
   const uint64_t row_bytes = row_vec * 16;
   // top halo = up neighbour's LAST row (its part 1); bottom halo = down neighbour's FIRST row (its part 0)
   const char* top = up_rank >= 0 ? slot_ptr(c, c.rank, rd, tensor_off, slot_bytes, up_rank) + (uint64_t)b * row_bytes : nullptr;

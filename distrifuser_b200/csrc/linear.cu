@@ -184,8 +184,8 @@ linear_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant__ 
             if (res) o = __hadd2(o, *reinterpret_cast<const __half2*>(res + c));   // torch: fp16 linear output, then fp16 add
             *reinterpret_cast<__half2*>(dst + c) = o;
             if (p.publish && col >= p.pub_col0) {          // k|v columns: also into every peer's slot of the publish epoch
-              const uint64_t off = (uint64_t)(pub_epoch % DF_NBANKS) * p.comm.bank_stride + p.tensor_off +
-                                   (uint64_t)p.comm.rank * p.slot_bytes + ((uint64_t)grow * p.pub_cols + (col - p.pub_col0)) * 2;
+              const uint64_t off = slot_offset(p.comm, pub_epoch, p.tensor_off, p.slot_bytes, p.comm.rank) +
+                                   ((uint64_t)grow * p.pub_cols + (col - p.pub_col0)) * 2;
               for (int q = 0; q < p.comm.world; ++q)
                 if (p.peer_mask >> q & 1) *reinterpret_cast<__half2*>((char*)p.comm.base[q] + off) = o;
             }
@@ -193,41 +193,13 @@ linear_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant__ 
         }
       }
     }
-    if (p.publish) __threadfence_system();                 // peer stores of this thread are visible system-wide before the ticket
   }
-  __syncthreads();
-  if (p.publish && threadIdx.x == 0) {
-    // last CTA of the grid stamps the peers' flags (same protocol as publish_kernel, csrc/comm.cu)
-    const uint32_t epoch = p.comm.clock[0];
-    __threadfence_system();
-    const uint32_t ticket = atomicAdd(&p.comm.tickets[p.idx], 1u);
-    if (ticket == gridDim.x - 1) {
-      __threadfence();
-      p.comm.tickets[p.idx] = 0;
-      for (int q = 0; q < p.comm.world; ++q)
-        if (p.peer_mask >> q & 1) st_release_sys(p.comm.flags[q] + (size_t)p.idx * p.comm.world + p.comm.rank, epoch);
-    }
-  }
-}
-
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                  const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-EncodeTiledFn get_encode2() {
-  static EncodeTiledFn fn = nullptr;
-  if (!fn) {
-    void* ptr = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &ptr, cudaEnableDefault, &q) == cudaSuccess && q == cudaDriverEntryPointSuccess)
-      fn = (EncodeTiledFn)ptr;
-  }
-  return fn;
+  if (p.publish) signal_when_last(p.comm, &p.comm.tickets[p.idx], gridDim.x, p.idx, p.peer_mask, p.comm.clock[0]);
 }
 
 // 2-D view [K (contiguous), rows] of a row-major [rows, pitch] fp16 matrix; box = [64, box_rows], 128B swizzle, zero fill
 int make_map2d(CUtensorMap* m, const void* base, int64_t rows, int K, int64_t pitch, int box_rows) {
-  EncodeTiledFn enc = get_encode2();
+  EncodeTiledFn enc = tensor_map_encoder();
   DF_REQUIRE(enc != nullptr, "cuTensorMapEncodeTiled is not available from this driver");
   cuuint64_t dims[2] = {(cuuint64_t)K, (cuuint64_t)rows};
   cuuint64_t strides[1] = {(cuuint64_t)pitch * 2};
@@ -264,11 +236,6 @@ double tile_cost(int64_t M, int N, int bn, int ctas_avail) {
 }  // namespace
 
 namespace {
-int sm_count_cached() {
-  static int sms = 0;
-  if (!sms) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev); if (sms <= 0) sms = kSmCount; }
-  return sms;
-}
 // tile width for a problem: 256, or 160 where that fills the SMs better (GEGLU: only widths that tile N exactly)
 int pick_bn(int64_t M, int N, int epilogue, int cap) {
   const bool ok160 = epilogue == EPI_PLAIN || N % 160 == 0, ok256 = epilogue == EPI_PLAIN || N % 256 == 0;
@@ -280,14 +247,14 @@ int pick_bn(int64_t M, int N, int epilogue, int cap) {
 
 extern "C" int df_linear_supported(int64_t M, int N, int K, int epilogue) {
   if (M < 1 || N < 8 || N % 8 != 0 || K < BK || K % BK != 0) return 0;
-  if (epilogue == EPI_GEGLU && pick_bn(M, N, epilogue, sm_count_cached()) == 0) return 0;   // blocks of 80 / 128 must tile N / 2
+  if (epilogue == EPI_GEGLU && pick_bn(M, N, epilogue, sm_count()) == 0) return 0;   // blocks of 80 / 128 must tile N / 2
   return 1;
 }
 
 // GEGLU epilogue: rows of the interleaved weight per hidden / gate block (= half the tile width chosen for this problem)
 extern "C" int df_linear_geglu_block(int64_t M, int N, int K) {
   (void)K;
-  const int bn = pick_bn(M, N, EPI_GEGLU, sm_count_cached());
+  const int bn = pick_bn(M, N, EPI_GEGLU, sm_count());
   return bn / 2;
 }
 
@@ -306,7 +273,7 @@ extern "C" int df_linear_fwd(df_comm_t comm, const void* a, const void* w, const
   memset(&args, 0, sizeof(args));
   args.bias = (const __half*)bias; args.residual = (const __half*)residual; args.out = (__half*)out;
   args.M = M; args.N = N; args.K = K; args.ldr = ldr; args.ldo = ldo;
-  const int sms = sm_count_cached();
+  const int sms = sm_count();
   const int cap = max_ctas > 0 ? max_ctas : sms;
   int bn = pick_bn(M, N, epilogue, epilogue == EPI_GEGLU ? sms : cap);   // GEGLU: must agree with df_linear_geglu_block()
   if (epilogue == EPI_GEGLU && geglu_block > 0) {

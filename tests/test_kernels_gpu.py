@@ -250,7 +250,7 @@ def _gn_call(x, G, w, b_, eps, mode, bessel, negfb, silu, comm, idx, off, sb, ma
 
 
 @pytest.mark.parametrize("B,Cc,H,W,G", [(2, 320, 32, 32, 32), (1, 640, 16, 24, 32), (2, 960, 8, 8, 32), (1, 1280, 15, 60, 32),
-                                       (2, 64, 8, 16, 32), (1, 2560, 4, 8, 32), (1, 80, 6, 10, 8)])
+                                       (2, 64, 8, 16, 32), (1, 2560, 4, 8, 32), (1, 80, 6, 10, 8), (5, 320, 96, 96, 32)])
 @pytest.mark.parametrize("silu", [0, 1])
 def test_groupnorm_local(B, Cc, H, W, G, silu):
     from distrifuser_b200 import _lib

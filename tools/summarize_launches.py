@@ -7,8 +7,7 @@ from collections import defaultdict
 
 def family(name: str) -> str:
     n = name
-    for pat, fam in ((r"fmha_fwd_kernel", "OURS fmha_fwd_kernel (wgmma)"), (r"gn_fused_kernel", "OURS gn_fused_kernel"), (r"gn_stats_kernel", "OURS gn_stats_kernel"),
-                     (r"gn_apply_kernel", "OURS gn_apply_kernel"), (r"gn_exchange_kernel", "OURS gn_exchange_kernel"),
+    for pat, fam in ((r"fmha_fwd_kernel", "OURS fmha_fwd_kernel (wgmma)"), (r"gn_fused_kernel", "OURS gn_fused_kernel"),
                      (r"halo_|publish_kernel|wait_kernel|step_begin|out_scatter|out_collect", "OURS comm/halo kernels"),
                      (r"geglu_kernel", "OURS geglu_kernel"), (r"add_layernorm_kernel", "OURS add_layernorm_kernel"),
                      (r"bias_residual_add_kernel", "OURS bias_residual_add_kernel (conv bias + residual)"),
