@@ -7,27 +7,9 @@ import ctypes as C
 import pytest
 import torch
 
-from helpers import LoopbackArena, sdpa_ref
+from helpers import LoopbackArena, _attn, _gn_call, _gn_ref, _moments, _sdpa_ref_chunked, sdpa_ref
 
 pytestmark = pytest.mark.gpu
-
-
-def _attn(q, kv, heads, comm=None, maps=None, nseg=1, own=0, idx=0, lseg=None, wait=0, no_ws=False):
-    from distrifuser_b200 import _lib
-    b, lq, Cq = q.shape
-    d = Cq // heads
-    out = torch.empty_like(q)
-    seg_rank = (C.c_int32 * 8)(*range(8))
-    L = _lib.lib()
-    # zeroed scratch: ticket counter of the dynamic schedule, partials of split units (no_ws: static whole-unit lists instead)
-    ws_bytes = 0 if no_ws else L.df_attn_workspace_bytes(b, lq, lseg or kv.shape[1], nseg, heads, d)
-    ws = torch.zeros(max(ws_bytes, 1), dtype=torch.uint8, device="cuda")
-    _lib.check(L.df_attn_fwd(comm or _lib.null_comm(), q.data_ptr(), kv.data_ptr(), out.data_ptr(), maps, b, lq,
-                             lseg or kv.shape[1], heads, d, q.stride(1), kv.stride(1), out.stride(1), nseg, own,
-                             seg_rank, idx, wait, 0.0, ws.data_ptr() if ws_bytes else None, ws_bytes,
-                             torch.cuda.current_stream().cuda_stream), "df_attn_fwd")
-    torch.cuda.synchronize()
-    return out
 
 
 @pytest.mark.parametrize("b,lq,lk,heads,d", [
@@ -181,14 +163,6 @@ def test_attention_multi_segment_stale_slots(n, own):
     assert err < 2e-3, f"max abs err {err}"
 
 
-def _sdpa_ref_chunked(q, k, v, heads, chunk=1800):
-    """fp32 reference for shapes whose [heads, lq, lk] score tensor does not fit: q rows in chunks."""
-    out = torch.empty(q.shape, dtype=torch.float32, device=q.device)
-    for r0 in range(0, q.shape[1], chunk):
-        out[:, r0:r0 + chunk] = sdpa_ref(q[:, r0:r0 + chunk], k, v, heads)
-    return out
-
-
 @pytest.mark.parametrize("lq,lseg,heads,own", [(3600, 3600, 20, 1),      # SDXL 3840^2, n=4, level 2 (Lkv 14 400)
                                                (14400, 14400, 10, 3)])   # SDXL 3840^2, n=4, level 1 (Lkv 57 600)
 def test_attention_3840_shapes_four_ragged_segments(lq, lseg, heads, own):
@@ -217,36 +191,6 @@ def test_attention_3840_shapes_four_ragged_segments(lq, lseg, heads, own):
     err = (out.float() - ref).abs().max().item()
     arena.close()
     assert err < 2e-3, f"max abs err {err}"
-
-
-def _gn_ref(x, G, w, b_, eps, mean, meansq, bessel=True, silu=False):
-    B, Cc, H, W = x.shape
-    x5 = x.float().view(B, G, Cc // G, H, W)
-    var = meansq - mean * mean
-    ne = (Cc // G) * H * W
-    if bessel:
-        var = var * (ne / (ne - 1))
-    y = ((x5 - mean) / (var + eps).sqrt()).view(B, Cc, H, W) * w.float().view(1, -1, 1, 1) + b_.float().view(1, -1, 1, 1)
-    return torch.nn.functional.silu(y) if silu else y
-
-
-def _moments(x, G):
-    B, Cc, H, W = x.shape
-    x5 = x.float().view(B, G, Cc // G, H, W)
-    return x5.mean(dim=[2, 3, 4], keepdim=True), (x5 * x5).mean(dim=[2, 3, 4], keepdim=True)
-
-
-def _gn_call(x, G, w, b_, eps, mode, bessel, negfb, silu, comm, idx, off, sb, mask, addend=None, apitch=0):
-    from distrifuser_b200 import _lib
-    L = _lib.lib()
-    B, Cc, H, W = x.shape
-    y = torch.empty_like(x, memory_format=torch.channels_last)
-    scratch = torch.zeros(L.df_groupnorm_scratch_bytes(B, G, H, W, Cc), dtype=torch.uint8, device="cuda")
-    _lib.check(L.df_groupnorm_fwd(comm, x.data_ptr(), addend.data_ptr() if addend is not None else None, apitch, y.data_ptr(), w.data_ptr(), b_.data_ptr(), B, H, W, Cc, G, eps, mode,
-                                  bessel, negfb, silu, idx, off, sb, mask, scratch.data_ptr(),
-                                  torch.cuda.current_stream().cuda_stream), "df_groupnorm_fwd")
-    torch.cuda.synchronize()
-    return y
 
 
 @pytest.mark.parametrize("B,Cc,H,W,G", [(2, 320, 32, 32, 32), (1, 640, 16, 24, 32), (2, 960, 8, 8, 32), (1, 1280, 15, 60, 32),

@@ -5,15 +5,9 @@ the k|v columns into the peers' arena slots.  Tolerance: fp16 storage of an fp32
 import pytest
 import torch
 
-from helpers import LoopbackArena
+from helpers import LoopbackArena, _close
 
 pytestmark = pytest.mark.gpu
-
-
-def _close(out, ref, rel=2e-3, abs_=4e-3):
-    err = (out.float() - ref).abs()
-    bad = err > (abs_ + rel * ref.abs())
-    assert not bad.any(), f"max err {err.max().item():.4e} at ref {ref.flatten()[err.flatten().argmax()].item():.3f}; {int(bad.sum())} bad"
 
 
 @pytest.mark.parametrize("M,N,K", [
