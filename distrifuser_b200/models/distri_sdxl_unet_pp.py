@@ -32,34 +32,67 @@ def _output_cls():
     return UNet2DConditionOutput
 
 
+def install_pp_wrappers(model: nn.Module, distri_config) -> None:
+    """Module surgery of distri_sdxl_unet_pp.py:19-40 in place: 3x3 convs, self / cross attention and GroupNorm become the
+    sm_90a wrappers, GroupNorm -> SiLU pairs fuse, and the UNet goes channels_last.  The wrappers read the patch layout from
+    `distri_config` (NaivePatchUNet passes a one-patch view of its config)."""
+    for name, module in list(model.named_modules()):
+        if isinstance(module, BaseModule):
+            continue
+        for subname, submodule in list(module.named_children()):
+            if isinstance(submodule, nn.Conv2d):
+                k = submodule.kernel_size
+                if k == (1, 1) or k == 1:
+                    continue
+                setattr(module, subname, DistriConv2dPP(submodule, distri_config, is_first_layer=subname == "conv_in"))
+            elif _is_attention(submodule):
+                if subname == "attn1":
+                    setattr(module, subname, DistriSelfAttentionPP(submodule, distri_config))
+                else:
+                    assert subname == "attn2"
+                    setattr(module, subname, DistriCrossAttentionPP(submodule, distri_config))
+            elif isinstance(submodule, nn.GroupNorm):
+                setattr(module, subname, DistriGroupNorm(submodule, distri_config))
+    # GroupNorm -> SiLU fusion where the block exposes the switch (compat UNet; diffusers blocks keep SiLU separate)
+    for module in model.modules():
+        if hasattr(module, "fused_norm_act"):
+            module.fused_norm_act = True
+            for nm in ("norm1", "norm2", "conv_norm_out"):
+                sub = getattr(module, nm, None)
+                if isinstance(sub, DistriGroupNorm):
+                    sub.fuse_silu = True
+    model.to(memory_format=torch.channels_last)
+
+
+def cfg_branch(cfg: DistriConfig, sample, timestep, encoder_hidden_states, added_cond_kwargs):
+    """This rank's half of the CFG batch (distri_sdxl_unet_pp.py:77-87 / 134-146)."""
+    i = cfg.batch_idx()
+    sample = sample[i:i + 1]
+    if torch.is_tensor(timestep) and timestep.ndim > 0:
+        timestep = timestep[i:i + 1]
+    encoder_hidden_states = encoder_hidden_states[i:i + 1]
+    if added_cond_kwargs is not None:                                # new dict: the caller's is not mutated (SURVEY D-10)
+        added_cond_kwargs = {k: v[i:i + 1] for k, v in added_cond_kwargs.items()}
+    return sample, timestep, encoder_hidden_states, added_cond_kwargs
+
+
+def load_static_inputs(si: dict, sample, timestep, encoder_hidden_states, added_cond_kwargs) -> None:
+    """Copies a call's inputs into the captured graphs' static inputs (distri_sdxl_unet_pp.py:89-106)."""
+    assert si["sample"].shape == sample.shape
+    si["sample"].copy_(sample)
+    if torch.is_tensor(timestep):
+        si["timestep"].copy_(timestep.expand(si["timestep"].shape) if timestep.ndim == 0 else timestep)
+    else:
+        si["timestep"].fill_(timestep)                               # no .item() host sync (SURVEY A6)
+    si["encoder_hidden_states"].copy_(encoder_hidden_states)
+    if added_cond_kwargs is not None:
+        for k in added_cond_kwargs:
+            si["added_cond_kwargs"][k].copy_(added_cond_kwargs[k])
+
+
 class DistriUNetPP(BaseModel):  # for Patch Parallelism
     def __init__(self, model: nn.Module, distri_config: DistriConfig):
-        for name, module in list(model.named_modules()):             # distri_sdxl_unet_pp.py:19-40
-            if isinstance(module, BaseModule):
-                continue
-            for subname, submodule in list(module.named_children()):
-                if isinstance(submodule, nn.Conv2d):
-                    k = submodule.kernel_size
-                    if k == (1, 1) or k == 1:
-                        continue
-                    setattr(module, subname, DistriConv2dPP(submodule, distri_config, is_first_layer=subname == "conv_in"))
-                elif _is_attention(submodule):
-                    if subname == "attn1":
-                        setattr(module, subname, DistriSelfAttentionPP(submodule, distri_config))
-                    else:
-                        assert subname == "attn2"
-                        setattr(module, subname, DistriCrossAttentionPP(submodule, distri_config))
-                elif isinstance(submodule, nn.GroupNorm):
-                    setattr(module, subname, DistriGroupNorm(submodule, distri_config))
-        # GroupNorm -> SiLU fusion where the block exposes the switch (compat UNet; diffusers blocks keep SiLU separate)
-        for module in model.modules():
-            if hasattr(module, "fused_norm_act"):
-                module.fused_norm_act = True
-                for nm in ("norm1", "norm2", "conv_norm_out"):
-                    sub = getattr(module, nm, None)
-                    if isinstance(sub, DistriGroupNorm):
-                        sub.fuse_silu = True
-        model.to(memory_format=torch.channels_last)
+        install_pp_wrappers(model, distri_config)
         super().__init__(model, distri_config)
 
     def _step_kind(self) -> int:
@@ -93,28 +126,13 @@ class DistriUNetPP(BaseModel):  # for Patch Parallelism
                 and mid_block_additional_residual is None and down_intrablock_additional_residuals is None
                 and encoder_attention_mask is None)                  # distri_sdxl_unet_pp.py:63-72
         split = cfg.world_size > 1 and cfg.do_classifier_free_guidance and cfg.split_batch
-        if split:                                                    # distri_sdxl_unet_pp.py:77-87 / 134-146
+        if split:
             assert b == 2
-            i = cfg.batch_idx()
-            sample = sample[i:i + 1]
-            if torch.is_tensor(timestep) and timestep.ndim > 0:
-                timestep = timestep[i:i + 1]
-            encoder_hidden_states = encoder_hidden_states[i:i + 1]
-            if added_cond_kwargs is not None:                        # new dict: the caller's is not mutated (SURVEY D-10)
-                added_cond_kwargs = {k: v[i:i + 1] for k, v in added_cond_kwargs.items()}
+            sample, timestep, encoder_hidden_states, added_cond_kwargs = cfg_branch(
+                cfg, sample, timestep, encoder_hidden_states, added_cond_kwargs)
 
         if cfg.use_cuda_graph and not record and self.cuda_graphs is not None:
-            si = self.static_inputs                                  # distri_sdxl_unet_pp.py:89-106
-            assert si["sample"].shape == sample.shape
-            si["sample"].copy_(sample)
-            if torch.is_tensor(timestep):
-                si["timestep"].copy_(timestep.expand(si["timestep"].shape) if timestep.ndim == 0 else timestep)
-            else:
-                si["timestep"].fill_(timestep)                       # no .item() host sync (SURVEY A6)
-            si["encoder_hidden_states"].copy_(encoder_hidden_states)
-            if added_cond_kwargs is not None:
-                for k in added_cond_kwargs:
-                    si["added_cond_kwargs"][k].copy_(added_cond_kwargs[k])
+            load_static_inputs(self.static_inputs, sample, timestep, encoder_hidden_states, added_cond_kwargs)
             if self.counter <= cfg.warmup_steps:                     # distri_sdxl_unet_pp.py:108-113
                 graph_idx = 0
             elif self.counter == cfg.warmup_steps + 1:

@@ -10,12 +10,15 @@ import os
 import torch
 
 from .models.distri_sdxl_unet_pp import DistriUNetPP
+from .models.naive_patch_sdxl import NaivePatchUNet
 from .utils import DistriConfig, PatchParallelismCommManager
 
 
 def _wrap(unet, distri_config: DistriConfig):
     if distri_config.parallelism == "patch":                         # pipelines.py:30-37
         return DistriUNetPP(unet, distri_config)
+    if distri_config.parallelism == "naive_patch":
+        return NaivePatchUNet(unet, distri_config)
     raise ValueError(f"Unknown / unsupported parallelism: {distri_config.parallelism}")
 
 
@@ -66,15 +69,19 @@ class _DistriPipelineBase:
             unet.set_counter(0)
             unet(**static_inputs, return_dict=False, record=True)    # registration pass (pipelines.py:138-139)
             comm_manager.create_buffer()                             # pipelines.py:140-141
-        unet.set_counter(0)
-        unet(**static_inputs, return_dict=False, record=True)        # pre-run (pipelines.py:144-145)
+        # pre-run (pipelines.py:144-145); naive patch also runs the column strip of its second graph eagerly, so that library
+        # autotuning and the wrappers' scratch allocations happen outside the capture
+        for counter in ([0, 1] if cfg.parallelism == "naive_patch" and cfg.split_scheme == "alternate" else [0]):
+            unet.set_counter(counter)
+            unet(**static_inputs, return_dict=False, record=True)
         self.static_inputs = static_inputs
         self.comm_manager = comm_manager
         self._capture_graphs()
 
     @torch.no_grad()
     def _capture_graphs(self):
-        """Three graphs: synchronous step, first asynchronous step, steady state (pipelines.py:147-165)."""
+        """Patch parallelism: three graphs, synchronous step, first asynchronous step, steady state.  Naive patch: the graphs
+        of counters 0 and 1, the row and column strips of `alternate` (pipelines.py:147-165)."""
         cfg, unet, static_inputs = self.distri_config, self.pipeline.unet, self.static_inputs
         static_outputs, cuda_graphs = [], []
         unet.setup_cuda_graph(None, None, None)
@@ -82,7 +89,10 @@ class _DistriPipelineBase:
             if self.comm_manager is not None:
                 self.comm_manager.clear()
             torch.cuda.synchronize()
-            counters = [0, cfg.warmup_steps + 1, cfg.warmup_steps + 2]
+            if cfg.parallelism == "naive_patch":
+                counters = [0, 1]
+            else:
+                counters = [0, cfg.warmup_steps + 1, cfg.warmup_steps + 2]
             unet.static_inputs = None
             pool = None
             from . import _lib
@@ -91,7 +101,9 @@ class _DistriPipelineBase:
             # stream's 0): when a K/V projection finishes, the attention grid that follows it takes the SM slots before the
             # publication kernel of the same K/V does -- a publication CTA that got there first keeps a persistent attention
             # CTA out of its SM for the whole transfer
-            prio = int(os.environ.get("DF_COMPUTE_PRIO", "-1" if cfg.n_device_per_batch > 1 else "0"))   # no publications without patch peers
+            # no publications without patch peers (one patch, or naive patch)
+            patch_peers = cfg.parallelism == "patch" and cfg.n_device_per_batch > 1
+            prio = int(os.environ.get("DF_COMPUTE_PRIO", "-1" if patch_peers else "0"))
             capture_stream = torch.cuda.Stream(device=cfg.device, priority=prio)
             for counter in counters:
                 graph = torch.cuda.CUDAGraph()
@@ -107,7 +119,9 @@ class _DistriPipelineBase:
 
     def set_mode(self, mode: str):
         """Switch the synchronisation mode (e.g. to "no_sync", the compute-only lower bound used for the exposed
-        communication metric, SURVEY 8d) on the same arena and re-capture the graphs."""
+        communication metric, SURVEY 8d) on the same arena and re-capture the graphs.  Patch parallelism only."""
+        if self.distri_config.parallelism != "patch":
+            raise ValueError(f"set_mode needs parallelism='patch', not {self.distri_config.parallelism!r}")
         self.distri_config.mode = mode
         self._capture_graphs()
 

@@ -54,10 +54,13 @@ class DistriConfig:
             f"distrifuser_b200 shards one image over the GPUs of ONE NVSwitch box (<= {_lib.MAX_WORLD} ranks, "
             f"DF_MAX_WORLD); got world_size={world_size}")
         assert mode in ("corrected_async_gn", "stale_gn", "sync_gn", "separate_gn", "full_sync", "no_sync")
-        if parallelism != "patch":
+        if parallelism == "naive_patch":
+            if split_scheme not in ("row", "col", "alternate"):                 # NaivePatchUNet.forward raises the same
+                raise NotImplementedError(f"naive_patch split_scheme must be row, col or alternate, got {split_scheme!r}")
+        elif parallelism != "patch":
             raise NotImplementedError(
-                "distrifuser_b200 implements the displaced patch-parallel path only (tensor / naive_patch are the "
-                "reference's comparison baselines and out of scope)")
+                "distrifuser_b200 implements displaced patch parallelism and the naive patch baseline (tensor parallelism "
+                "is out of scope)")
 
         self.world_size = world_size
         self.rank = rank
@@ -80,6 +83,12 @@ class DistriConfig:
         else:
             n_device_per_batch = world_size
         self.n_device_per_batch = n_device_per_batch
+        if parallelism == "naive_patch":
+            # every rank runs the UNet on a strip of whole latent rows / columns (alternate: both, one per step)
+            rows_ok, cols_ok = height % (8 * n_device_per_batch) == 0, width % (8 * n_device_per_batch) == 0
+            if not {"row": rows_ok, "col": cols_ok, "alternate": rows_ok and cols_ok}[split_scheme]:
+                raise ValueError(f"naive_patch {split_scheme} split of a {height}x{width} image over {n_device_per_batch} "
+                                 f"ranks: the {height // 8}x{width // 8} latent does not split into whole strips")
 
         if torch.cuda.is_available():
             ndev = torch.cuda.device_count()
@@ -302,7 +311,8 @@ class PatchParallelismCommManager:
     # acknowledgement.  That is safe only because every UNet call ends with df_output_gather, which makes each rank wait
     # for the epsilon strip of EVERY world rank: no rank can start call t+1 before all ranks finished the kernels of call
     # t, so ranks drift by < 1 call and a store of epoch e+3 can never meet a read of epoch e (reads of epoch e happen in
-    # calls e and e+1 only).  A path that skips the gather (e.g. returning the local strip) must add its own per-call
+    # calls e and e+1 only).  NaivePatchUNet ends every call with the same world gather (df_output_gather_2d), so its output
+    # banks obey the same bound.  A path that skips the gather (e.g. returning the local strip) must add its own per-call
     # world barrier, or stale K/V / halo rows get corrupted silently.
     def step_begin(self, kind: int):
         """kind 0 = synchronous, 1 = asynchronous, 2 = frozen (see df_step_begin)."""

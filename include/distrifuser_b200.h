@@ -156,6 +156,13 @@ int df_attn_fwd(df_comm_t comm, const void* q, const void* kv_own, void* out, co
 int df_output_gather(df_comm_t comm, const void* strip, void* out, int B, int C, int H, int W, int bs, int hs,
                      int batch0, int row0, int idx, uint64_t tensor_off, void* stream);
 
+/* Same gather for a strip that need not span the full width: replaces the all_gather + cat(dim=2 or 3) of
+ * NaivePatchUNet.forward (distrifuser/models/naive_patch_sdxl.py:151-154,195-197).  strip: [bs,C,hs,ws] NCHW fp16,
+ * placed at batch `batch0`, row `row0`, column `col0` of the [B,C,H,W] image.  16-byte stores when ws, col0 and W are
+ * multiples of 8 (or ws == W and hs*W is), 2-byte stores otherwise. */
+int df_output_gather_2d(df_comm_t comm, const void* strip, void* out, int B, int C, int H, int W, int bs, int hs, int ws,
+                        int batch0, int row0, int col0, int idx, uint64_t tensor_off, void* stream);
+
 /* ---- fused GEGLU gate of the transformer feed-forward: out[r, c] = in[r, c] * gelu_erf(in[r, cols + c]).
  *      Not one of the reference's wrapped modules (diffusers FeedForward, SURVEY Appendix A) but on the per-step
  *      path inside DistriUNetPP.forward; in:[rows, 2*cols] fp16 (pitch in_pitch elements), out:[rows, cols]. ---- */
