@@ -7,17 +7,20 @@
 //     F.scaled_dot_product_attention -> S = Q K^T and O += P V as wgmma tiles, accumulators in registers
 // and the SDPA of DistriCrossAttentionPP.forward (attn.py:79-87) with nseg = 1, lseg = 77.
 //
-// Persistent CTAs (288 threads: two consumer warpgroups + one producer warp; one CTA per SM)
+// Persistent CTAs (384 threads: two consumer warpgroups + one producer warpgroup; one CTA per SM)
 // walk work items = one 128-row Q tile of one (batch, head), or a K/V range of one:
-//   warps 0-7  two consumer warpgroups, 64 Q rows each.  Per K/V tile: S = Q K^T (m64nSNk16 wgmmas, both operands in shared
-//              memory) into SN/2 fp32 registers per thread, online softmax on that fragment (a row lives in one quad: row maxima
-//              and sums are two shuffles; exp2 on MUFU with 3 of 16 column groups on a polynomial on the FMA pipe; the exponent
-//              reference only moves when the row maximum grew by more than 2^8), P packed to fp16 IN REGISTERS as the A operand of
-//              O += P V (m64n64k16 wgmmas, V MN-major from shared memory), O in registers; epilogue O / l -> HBM (or fp32
-//              partials merged by the last part of a split unit)
-//   warp 8     scheduler + TMA producer: hands out work items through a two-entry ring (whole units drawn from an atomic ticket
-//              counter when the grid fills the SMs, a static one-item list otherwise), then Q per item and K (KST stages) /
-//              V (VST stages) tiles through mbarrier rings; waits the peers' flags
+//   warps 0-7  two consumer warpgroups, 64 Q rows each.  Per S slice (SN K/V rows): S = Q K^T (m64nSNk16 wgmmas, both operands
+//              in shared memory) into SN/2 fp32 registers per thread, online softmax on that fragment (a row lives in one quad:
+//              row maxima and sums are two shuffles; exp2 on MUFU with 3 of 16 column groups on a polynomial on the FMA pipe; the
+//              exponent reference only moves when the row maximum grew by more than 2^8), P packed to fp16 IN REGISTERS as the A
+//              operand of O += P V (m64n64k16 wgmmas, V MN-major from shared memory), O in registers; epilogue O / l -> HBM (or
+//              fp32 partials merged by the last part of a split unit).  At d <= 80 the MMAs of slice i + 1's S and slice i's
+//              P V are issued together, so the softmax of slice i + 1 runs while the tensor cores compute P_i V_i, and the two
+//              warpgroups take turns on the tensor cores (Cfg::OVERLAP / PINGPONG).
+//   warps 8-11 producer warpgroup (gives its registers to the consumers); lane 0 of warp 8 is the scheduler + TMA producer: hands
+//              out work items through a two-entry ring (whole units drawn from an atomic ticket counter when the grid fills the
+//              SMs, a static one-item list otherwise), then Q per item and K (KST stages) / V (VST stages) tiles through mbarrier
+//              rings; waits the peers' flags
 
 #include "tc_ptx.cuh"
 
@@ -30,8 +33,10 @@ constexpr int BM = 128;      // Q rows per CTA (64 per consumer warpgroup)
 constexpr int BN = 128;      // K/V rows per tile
 constexpr int HB = 64;       // head-dim block: one 128-byte swizzled row; d is padded to NBLK * 64 columns (TMA zero-fills)
 constexpr int NCONSUMER_WARPS = 8;
-constexpr int NTHREADS = 32 * (NCONSUMER_WARPS + 1);
+constexpr int NTHREADS = 32 * (NCONSUMER_WARPS + 4);
 constexpr int WARP_TMA = NCONSUMER_WARPS;
+// registers per thread after setmaxnreg: 128 x PRODUCER_REGS + 256 x CONSUMER_REGS <= 65536
+constexpr int PRODUCER_REGS = 56, CONSUMER_REGS = 224;    // the producer lane spills below 56
 constexpr uint32_t BLK_BYTES = BN * HB * 2;                // one 128 x 64 fp16 block = 16 KiB
 
 // NBLK = ceil(d / 64): 1 for d in {40, 64} (SDXL, SD1.x level 0), 2 for d = 80, 3 for d = 160 (SD1.x)
@@ -46,13 +51,18 @@ struct __align__(1024) SmemT {
   int sched_code[2];
   uint32_t ticket;            // arrival ticket of this part among the parts of its left-over unit
 };
-// One CTA per SM.  Registers of a kernel that issues wgmma are allocated per warpgroup, so the producer warp costs a whole
-// warpgroup's share and a thread gets at most 168 (65536 / 384): the S slice (SN / 2), the O fragment (32 per head block) and
-// the packed P (SN / 4) must fit in that -- hence 128-wide S slices at d <= 64 and 64-wide ones for the wider heads.
+// One CTA per SM.  A consumer thread holds the S slice (SN / 2), the O fragment (32 per head block) and the packed P (SN / 4) in
+// at most CONSUMER_REGS registers: 128-wide S slices at d <= 64, 64-wide ones for the wider heads.  Shared memory (227 KiB)
+// sets the stage counts.  OVERLAP picks the order inside a warpgroup (see the consumer loop): serial (S, softmax, P V, wait)
+// or S of slice i + 1 issued with P V of slice i; PINGPONG (overlapped order only) hands the tensor cores to the two
+// warpgroups in turns.  The overlapped order frees a V stage one slice later, so it needs a spare V stage: d = 160 has room
+// for one only and keeps the serial order.  Without the turns the overlapped order was slower than the serial one at d <= 64
+// (both warpgroups wait on the same K tile and then run their softmax at the same time); with them it is faster (DESIGN §3.1).
 template <int NBLK> struct Cfg;
-template <> struct Cfg<1> { static constexpr int KST = 3, VST = 2, SN = 128; };
-template <> struct Cfg<2> { static constexpr int KST = 2, VST = 2, SN = 64; };
-template <> struct Cfg<3> { static constexpr int KST = 2, VST = 1, SN = 64; };
+template <> struct Cfg<1> { static constexpr int KST = 4, VST = 4, SN = 128; static constexpr bool OVERLAP = true, PINGPONG = true; };
+template <> struct Cfg<2> { static constexpr int KST = 3, VST = 3, SN = 64; static constexpr bool OVERLAP = true, PINGPONG = true; };
+template <> struct Cfg<3> { static constexpr int KST = 2, VST = 1, SN = 64; static constexpr bool OVERLAP = false, PINGPONG = false; };
+constexpr int TURN_BAR = 2;   // named barriers TURN_BAR + wg: the tensor-core turns of the two warpgroups (1: split merge)
 
 // work schedule of one launch (host: plan_schedule): every CTA takes `a` whole units; the R left-over units are cut into P parts
 struct Sched {
@@ -92,6 +102,7 @@ fmha_fwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
   constexpr int KSTAGES = Cfg<NBLK>::KST, VSTAGES = Cfg<NBLK>::VST;
   constexpr uint32_t TILE_BYTES = NBLK * BLK_BYTES;
   constexpr int SN = Cfg<NBLK>::SN, NSUB = BN / SN;
+  constexpr bool OVERLAP = Cfg<NBLK>::OVERLAP, PINGPONG = Cfg<NBLK>::PINGPONG;
   using Smem = SmemT<NBLK, KSTAGES, VSTAGES>;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   Smem& sm = *reinterpret_cast<Smem*>(smem_raw);
@@ -145,9 +156,10 @@ fmha_fwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
   __syncthreads();
   pdl_wait();                                          // everything above overlapped the tail of the previous kernel
 
-  if (warp == WARP_TMA) {
+  if (warp >= WARP_TMA) {
     // =============================================================== scheduler + TMA producer
-    if (lane == 0) {
+    setmaxnreg_dec<PRODUCER_REGS>();
+    if (warp == WARP_TMA && lane == 0) {
       prefetch_tmap(&tm_q);
       prefetch_tmap(&tm_kv_own);
       uint32_t rd = 0;
@@ -191,7 +203,7 @@ fmha_fwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
           if (seg != own_seg) {
             const int r = segs.rank[seg];
             if ((t == 0 || j == 0) && wait_flags) {
-              spin_until(flag_ptr(comm, comm.rank, idx, r), rd, comm.spin_timeout_ns);
+              spin_until<false>(flag_ptr(comm, comm.rank, idx, r), rd, comm.spin_timeout_ns);
               // the acquire above is a generic-proxy read; the peers' rows are fetched next through the async proxy (TMA)
               asm volatile("fence.proxy.async.global;" ::: "memory");
             }
@@ -213,15 +225,34 @@ fmha_fwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
     // =============================================================== consumers (warps 0-7): S, softmax, P V, epilogue
     // Warpgroup wg owns Q rows [64 wg, 64 wg + 64).  In the wgmma accumulator fragment thread t of warp w holds rows
     // rA = 64 wg + 16 (w & 3) + t/4 and rB = rA + 8, columns 8i + 2(t%4) + {0,1}: s[4i + {0,1}] (row rA), s[4i + {2,3}] (row rB).
+    setmaxnreg_inc<CONSUMER_REGS>();
     const int wg = warp >> 2;
     const int c4 = lane & 3;
     const int rowA = wg * 64 + (warp & 3) * 16 + (lane >> 2);
     const uint32_t q_base = smem_u32(sm.q) + wg * 64 * 128;
     uint32_t g = 0;                                                // K/V tiles processed so far by this CTA (barrier phases)
+    // Ping-pong: a warpgroup issues its MMAs of a slice only in its turn (named barrier TURN_BAR + wg) and then hands the turn
+    // to the other one, so one warpgroup's softmax runs under the other's MMAs instead of both waiting on the same tiles in
+    // step.  Both warpgroups take the same number of turns (they walk the same items and slices); warpgroup 0 takes the first
+    // turn, and its final sync below consumes warpgroup 1's last hand-over.
+    auto turn_begin = [&]() {
+      if constexpr (PINGPONG) {
+        if (wg == 0) named_bar_sync<TURN_BAR, 256>(); else named_bar_sync<TURN_BAR + 1, 256>();
+      }
+    };
+    auto turn_end = [&]() {
+      if constexpr (PINGPONG) {
+        if (wg == 0) named_bar_arrive<TURN_BAR + 1, 256>(); else named_bar_arrive<TURN_BAR, 256>();
+      }
+    };
+    if (PINGPONG && wg == 1) named_bar_arrive<TURN_BAR, 256>();
     for (uint32_t ui = 0;; ++ui) {
       mbar_wait(&sm.sched_full[ui & 1u], (ui >> 1) & 1u);
       const int code = *(volatile int*)&sm.sched_code[ui & 1u];
-      if (code == ITEM_END) break;
+      if (code == ITEM_END) {
+        if (PINGPONG && wg == 0) named_bar_sync<TURN_BAR, 256>();
+        break;
+      }
       int q0, head, bat, j_begin, T, slot, lo;
       decode(code, q0, head, bat, j_begin, T, slot, lo);
       // exponent references of rows rA / rB, kept NEGATED and in log2 units: P = 2^(S * scale_log2 + n)
@@ -230,29 +261,57 @@ fmha_fwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
       float o[NBLK * 32];
 #pragma unroll
       for (int i = 0; i < NBLK * 32; ++i) o[i] = 0.f;
+      float s[SN / 2];                                             // S of the current slice, then its P in fp32
+      uint32_t pk[SN / 4];                                         // P of a slice packed to fp16: the A operand of its P V
+      auto issue_s = [&](uint32_t ks, int sub) {                   // S = Q K^T of slice `sub` of K stage ks
+        const uint32_t k_addr = smem_u32(sm.k[ks]) + sub * SN * 128;
+        wgmma_fence();
+#pragma unroll
+        for (int blk = 0; blk < NBLK; ++blk)
+#pragma unroll
+          for (int kk = 0; kk < HB / 16; ++kk)
+            wgmma_ss<SN>(s, smem_desc(q_base + blk * BLK_BYTES + kk * 32, 16, 1024), smem_desc(k_addr + blk * BLK_BYTES + kk * 32, 16, 1024),
+                         (blk | kk) > 0);
+        wgmma_commit();
+      };
+      auto issue_pv = [&](uint32_t vs, int sub) {                  // O += P V of slice `sub` of V stage vs
+        const uint32_t v_addr = smem_u32(sm.v[vs]) + sub * SN * 128;
+        wgmma_fence();
+#pragma unroll
+        for (int kk = 0; kk < SN / 16; ++kk)
+#pragma unroll
+          for (int blk = 0; blk < NBLK; ++blk)
+            wgmma_rs_n64(o + 32 * blk, pk + 4 * kk, smem_desc(v_addr + blk * BLK_BYTES + kk * 2048, 16384, 1024), 1u);
+        wgmma_commit();
+      };
       mbar_wait(&sm.q_full, ui & 1u);
+      // The item's K/V tiles are processed in NSUB column slices of SN K/V rows (online softmax per slice): for the wider heads
+      // two slices of 64 keep the S fragment at 32 registers next to the larger O fragment.  Overlapped order, per slice i:
+      //   issue S_i = Q K_i^T and O += P_{i-1} V_{i-1} (two commit groups) -> wait<1> (S_i retired) -> row maxima, exp2, sums
+      //   of S_i in place -> wait<0> (P V retired) -> rescale O if slice i moved the reference -> pack P_i
+      // and the last slice's P V after the loop.  P_{i-1} stays in `pk` until its P V retires; the tensor cores run P V while
+      // this warpgroup runs the softmax.
       int t = j_begin % tps;
       for (int j = 0; j < T; ++j, ++t, ++g) {
         if (t == tps) t = 0;
         const int valid = min(BN, lseg - t * BN);
         const uint32_t ks = g % KSTAGES, vs = g % VSTAGES;
-        // The tile is processed in NSUB column slices of SN K/V rows (online softmax per slice): for the wider heads two slices of
-        // 64 keep the S fragment at 32 registers next to the larger O fragment.
 #pragma unroll
         for (int sub = 0; sub < NSUB; ++sub) {
-          // ---- S = Q K_j^T (this slice)
-          float s[SN / 2];
+          // ---- S = Q K_j^T (this slice), and the previous slice's P V
           if (sub == 0) mbar_wait(&sm.k_full[ks], (g / KSTAGES) & 1u);
-          const uint32_t k_addr = smem_u32(sm.k[ks]) + sub * SN * 128;
-          wgmma_fence();
-#pragma unroll
-          for (int blk = 0; blk < NBLK; ++blk)
-#pragma unroll
-            for (int kk = 0; kk < HB / 16; ++kk)
-              wgmma_ss<SN>(s, smem_desc(q_base + blk * BLK_BYTES + kk * 32, 16, 1024), smem_desc(k_addr + blk * BLK_BYTES + kk * 32, 16, 1024),
-                           (blk | kk) > 0);
-          wgmma_commit();
-          wgmma_wait<0>();
+          const bool pv = OVERLAP && (j > 0 || sub > 0);
+          const int subp = sub > 0 ? sub - 1 : NSUB - 1;             // the previous slice: tile gp, slice subp
+          const uint32_t gp = sub > 0 ? g : g - 1u, vsp = gp % VSTAGES;
+          if (pv && subp == 0) mbar_wait(&sm.v_full[vsp], (gp / VSTAGES) & 1u);
+          turn_begin();
+          issue_s(ks, sub);
+          // Always two commit groups in the overlapped order (an empty one when there is no previous slice): with the same
+          // wait counts on every path ptxas keeps the wgmmas asynchronous instead of serialising them (C7514 / C7515).
+          if (pv) issue_pv(vsp, subp);
+          else if (OVERLAP) wgmma_commit();
+          turn_end();
+          wgmma_wait<OVERLAP ? 1 : 0>();
           fence_regs<SN / 2>(s);
           if (sub == NSUB - 1) {
             __syncwarp();
@@ -284,49 +343,68 @@ fmha_fwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
           mA = fmaxf(mA, __shfl_xor_sync(0xffffffffu, mA, 2));
           mB = fmaxf(mB, __shfl_xor_sync(0xffffffffu, mB, 2));
           const float dA = fmaf(mA, scale_log2, nA), dB = fmaf(mB, scale_log2, nB);    // log2 of the largest P of the slice
-          if (dA > 8.f) {
-            const float alpha = ex2(-dA);
-            nA = -mA * scale_log2; lA *= alpha;
-#pragma unroll
-            for (int i = 0; i < NBLK * 8; ++i) { o[4 * i] *= alpha; o[4 * i + 1] *= alpha; }
-          }
-          if (dB > 8.f) {
-            const float alpha = ex2(-dB);
-            nB = -mB * scale_log2; lB *= alpha;
-#pragma unroll
-            for (int i = 0; i < NBLK * 8; ++i) { o[4 * i + 2] *= alpha; o[4 * i + 3] *= alpha; }
-          }
-          // ---- P = 2^(S * scale_log2 + n), row sums, packed to fp16 as the A fragment of the P V wgmmas
-          uint32_t pk[SN / 4];
+          const bool moveA = dA > 8.f, moveB = dB > 8.f;
+          float alphaA = 1.f, alphaB = 1.f;                // O's rescale waits for the P V in flight (it accumulates into O)
+          if (moveA) { alphaA = ex2(-dA); nA = -mA * scale_log2; lA *= alphaA; }
+          if (moveB) { alphaB = ex2(-dB); nB = -mB * scale_log2; lB *= alphaB; }
+          // ---- P = 2^(S * scale_log2 + n) in place, row sums
 #pragma unroll
           for (int i = 0; i < SN / 8; ++i) {
             const int grp = sub * (SN / 8) + i;            // column group of the 128-wide tile row
-            float e[4];
 #pragma unroll
             for (int k = 0; k < 4; ++k) {
               const float x = fmaf(s[4 * i + k], scale_log2, k < 2 ? nA : nB);
-              e[k] = ((grp * DF_EMU_GROUPS) / 16 != ((grp + 1) * DF_EMU_GROUPS) / 16) ? ex2_poly(x) : ex2(x);
+              s[4 * i + k] = ((grp * DF_EMU_GROUPS) / 16 != ((grp + 1) * DF_EMU_GROUPS) / 16) ? ex2_poly(x) : ex2(x);
             }
-            lA += e[0] + e[1];
-            lB += e[2] + e[3];
-            pk[2 * i] = pack_h2(e[0], e[1]);
-            pk[2 * i + 1] = pack_h2(e[2], e[3]);
+            lA += s[4 * i] + s[4 * i + 1];
+            lB += s[4 * i + 2] + s[4 * i + 3];
           }
-          // ---- O += P V_j (this slice's K/V rows)
-          if (sub == 0) mbar_wait(&sm.v_full[vs], (g / VSTAGES) & 1u);
-          const uint32_t v_addr = smem_u32(sm.v[vs]) + sub * SN * 128;
-          wgmma_fence();
+          if (OVERLAP) {
+            wgmma_wait<0>();
+            fence_regs<NBLK * 32>(o);
+          }
+          if (pv) {                                        // the previous slice's P V has retired: its V stage and `pk` are free
+            if (subp == NSUB - 1) {
+              __syncwarp();
+              if (lane == 0) mbar_arrive(&sm.v_empty[vsp]);
+            }
+          }
+          if (moveA) {
 #pragma unroll
-          for (int kk = 0; kk < SN / 16; ++kk)
+            for (int i = 0; i < NBLK * 8; ++i) { o[4 * i] *= alphaA; o[4 * i + 1] *= alphaA; }
+          }
+          if (moveB) {
 #pragma unroll
-            for (int blk = 0; blk < NBLK; ++blk)
-              wgmma_rs_n64(o + 32 * blk, pk + 4 * kk, smem_desc(v_addr + blk * BLK_BYTES + kk * 2048, 16384, 1024), 1u);
-          wgmma_commit();
-          wgmma_wait<0>();
-          fence_regs<NBLK * 32>(o);
+            for (int i = 0; i < NBLK * 8; ++i) { o[4 * i + 2] *= alphaB; o[4 * i + 3] *= alphaB; }
+          }
+          // ---- P packed to fp16 as the A fragment of the P V wgmmas
+#pragma unroll
+          for (int i = 0; i < SN / 8; ++i) {
+            pk[2 * i] = pack_h2(s[4 * i], s[4 * i + 1]);
+            pk[2 * i + 1] = pack_h2(s[4 * i + 2], s[4 * i + 3]);
+          }
+          if constexpr (!OVERLAP) {                        // serial order: O += P V_j (this slice) right away
+            if (sub == 0) mbar_wait(&sm.v_full[vs], (g / VSTAGES) & 1u);
+            issue_pv(vs, sub);
+            wgmma_wait<0>();
+            fence_regs<NBLK * 32>(o);
+            if (sub == NSUB - 1) {
+              __syncwarp();
+              if (lane == 0) mbar_arrive(&sm.v_empty[vs]);
+            }
+          }
         }
+      }
+      if constexpr (OVERLAP) {                             // P V of the item's last slice (tile g - 1, slice NSUB - 1)
+        const uint32_t vsp = (g - 1u) % VSTAGES;
+        if (NSUB == 1) mbar_wait(&sm.v_full[vsp], ((g - 1u) / VSTAGES) & 1u);
+        turn_begin();
+        issue_pv(vsp, NSUB - 1);
+        turn_end();
+        wgmma_wait<0>();
+        fence_regs<NBLK * 32>(o);
         __syncwarp();
-        if (lane == 0) mbar_arrive(&sm.v_empty[vs]);
+        if (lane == 0) mbar_arrive(&sm.v_empty[vsp]);
       }
       // ---- epilogue: quad-reduce the row sums, then O / l -> fp16 -> HBM (or an fp32 partial of a split unit)
       lA += __shfl_xor_sync(0xffffffffu, lA, 1); lB += __shfl_xor_sync(0xffffffffu, lB, 1);

@@ -67,6 +67,9 @@ __device__ __forceinline__ uint64_t globaltimer_ns() {
 #ifndef DF_SPIN_TIMEOUT_NS
 #define DF_SPIN_TIMEOUT_NS 30000000000ull  // a peer that never arrives becomes a CUDA error, not a hung GPU
 #endif
+// kReport = false drops the printf before the trap: a kernel that issues wgmma must contain no function call (printf is one),
+// or ptxas serialises every wgmma of the kernel (warning C7510).
+template <bool kReport = true>
 __device__ __forceinline__ void spin_until(const uint32_t* flag, uint32_t want, uint64_t timeout_ns = 0) {
   if (epoch_reached(ld_acquire_sys(flag), want)) return;
   if (timeout_ns == 0) timeout_ns = DF_SPIN_TIMEOUT_NS;
@@ -75,7 +78,8 @@ __device__ __forceinline__ void spin_until(const uint32_t* flag, uint32_t want, 
   while (!epoch_reached(ld_acquire_sys(flag), want)) {
     __nanosleep(64);
     if ((++polls & 1023u) == 0 && globaltimer_ns() - t0 > timeout_ns) {
-      printf("distrifuser_b200: timeout waiting for flag %p (have %u, want %u)\n", (const void*)flag, ld_volatile_u32(flag), want);
+      if constexpr (kReport)
+        printf("distrifuser_b200: timeout waiting for flag %p (have %u, want %u)\n", (const void*)flag, ld_volatile_u32(flag), want);
       __trap();
     }
   }

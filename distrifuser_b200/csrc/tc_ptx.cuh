@@ -85,6 +85,17 @@ __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.a
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 template <int N>
 __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// per-thread register budget of the calling warpgroup (every warp of the warpgroup executes it): a producer warpgroup hands
+// registers back to the pool, the consumer warpgroups take them (blocks until the pool has them)
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
+// named barriers (id 0 is __syncthreads): `count` threads take part, the arriving ones do not wait
+template <int ID, int COUNT>
+__device__ __forceinline__ void named_bar_sync() { asm volatile("bar.sync %0, %1;" ::"n"(ID), "n"(COUNT) : "memory"); }
+template <int ID, int COUNT>
+__device__ __forceinline__ void named_bar_arrive() { asm volatile("bar.arrive %0, %1;" ::"n"(ID), "n"(COUNT) : "memory"); }
 // keeps the compiler from touching accumulator registers across an asynchronous wgmma (issue ... wait)
 template <int N>
 __device__ __forceinline__ void fence_regs(float* d) {
