@@ -78,8 +78,12 @@ __device__ __forceinline__ float2 ld_f2(const float2* p) {          // coherent 
   return r;
 }
 
+// K/V segment layout of a launch.  Segments may have different lengths (uneven row strips of patch parallelism); the
+// kernel walks them in ORDER o = 0 .. nseg - 1, segment (own_seg + o) mod nseg, so that the own fresh segment comes first.
 struct SegInfo {
-  int32_t rank[DF_MAX_WORLD];  // world rank holding segment s
+  int32_t rank[DF_MAX_WORLD];      // world rank holding segment s
+  int32_t len[DF_MAX_WORLD];       // K/V rows of the segment at walk order o
+  int32_t tile0[DF_MAX_WORLD + 1]; // first tile of walk order o in the concatenated tile range; tile0[nseg] = all tiles
 };
 
 #ifndef DF_EMU_GROUPS
@@ -96,8 +100,8 @@ __device__ __forceinline__ void wgmma_ss(float* d, uint64_t a_desc, uint64_t b_d
 template <int NBLK>
 __global__ void __launch_bounds__(NTHREADS, 1)
 fmha_fwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant__ CUtensorMap tm_kv_own,
-                const CUtensorMap* __restrict__ kvmaps, df_comm_t comm, SegInfo segs, __half* __restrict__ out, int lq,
-                int lseg, int heads, int d, int64_t o_pitch, int nseg, int own_seg, int idx, int wait_flags,
+                const CUtensorMap* __restrict__ kvmaps, df_comm_t comm, const __grid_constant__ SegInfo segs, __half* __restrict__ out, int lq,
+                int heads, int d, int64_t o_pitch, int nseg, int own_seg, int idx, int wait_flags,
                 float scale_log2, Sched sched, float* part_o, float2* part_ml, unsigned int* part_cnt, unsigned int* sched_ctr) {
   constexpr int KSTAGES = Cfg<NBLK>::KST, VSTAGES = Cfg<NBLK>::VST;
   constexpr uint32_t TILE_BYTES = NBLK * BLK_BYTES;
@@ -118,8 +122,17 @@ fmha_fwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
   // tensor-map fetch and pipeline fill are paid once per CTA, and the K/V loads of the next item run under the epilogue of the
   // current one.
   const int nqt = (lq + BM - 1) / BM;
-  const int tps = (lseg + BN - 1) / BN;  // tiles per segment
-  const int T_all = nseg * tps;
+  const int T_all = segs.tile0[nseg];    // K/V tiles of all segments (each segment's last tile may be ragged)
+  const int tiles_own = segs.tile0[1], len_own = segs.len[0];     // the own segment (walk order 0), kept in registers
+  // walk order, tile inside that segment, its tile count and length for concatenated tile j (once per item, outside the tile
+  // loops).  Whole units start in the own segment and need no parameter loads; only split parts may start further on.
+  auto locate = [&](int j, int& so, int& t, int& tseg, int& lseg) {
+    so = 0; t = j; tseg = tiles_own; lseg = len_own;
+    if (j >= tiles_own) {
+      while (so + 1 < nseg && segs.tile0[so + 1] <= j) ++so;
+      t = j - segs.tile0[so]; tseg = segs.tile0[so + 1] - segs.tile0[so]; lseg = segs.len[so];
+    }
+  };
   const int n_items = sched.a + ((int)blockIdx.x < sched.R * sched.P ? 1 : 0);     // static schedule only
   // item code (from the ring, see the scheduler in the TMA lane) -> Q tile origin, head, batch, first K/V tile, tile count,
   // partial slot (-1: whole unit), left-over index.  Dynamic schedule: the code is the unit; static: the index into this
@@ -194,9 +207,10 @@ fmha_fwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
         mbar_expect_tx(&sm.q_full, TILE_BYTES);
 #pragma unroll
         for (int blk = 0; blk < NBLK; ++blk) tma_load_4d(sm.q[blk], &tm_q, &sm.q_full, blk * HB, head, q0, bat);
-        int so = j_begin / tps, t = j_begin - so * tps;   // segment order index, tile inside the segment (one division, outside the loop)
+        int so, t, tseg, lseg;                            // segment walk order, tile inside it, its tiles and rows
+        locate(j_begin, so, t, tseg, lseg);
         for (int j = 0; j < T; ++j, ++t, ++g) {
-          if (t == tps) { t = 0; ++so; }
+          if (t == tseg) { t = 0; ++so; tseg = segs.tile0[so + 1] - segs.tile0[so]; }
           int seg = own_seg + so;
           if (seg >= nseg) seg -= nseg;
           const void* map = &tm_kv_own;
@@ -291,9 +305,10 @@ fmha_fwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
       //   of S_i in place -> wait<0> (P V retired) -> rescale O if slice i moved the reference -> pack P_i
       // and the last slice's P V after the loop.  P_{i-1} stays in `pk` until its P V retires; the tensor cores run P V while
       // this warpgroup runs the softmax.
-      int t = j_begin % tps;
+      int so, t, tseg, lseg;                                       // segment walk order, tile inside it, its tiles and rows
+      locate(j_begin, so, t, tseg, lseg);
       for (int j = 0; j < T; ++j, ++t, ++g) {
-        if (t == tps) t = 0;
+        if (t == tseg) { t = 0; ++so; tseg = segs.tile0[so + 1] - segs.tile0[so]; lseg = segs.len[so]; }
         const int valid = min(BN, lseg - t * BN);
         const uint32_t ks = g % KSTAGES, vs = g % VSTAGES;
 #pragma unroll
@@ -498,23 +513,35 @@ int make_map(CUtensorMap* m, const void* base, int d, int nheads, int rows, int 
 
 }  // namespace
 
-extern "C" int df_attn_make_kvmaps(df_comm_t comm, uint64_t tensor_off, uint64_t slot_bytes, int b, int lseg, int heads,
-                                   int d, void* maps_out, void* stream) {
+// Tensor maps of every (bank, member) slot of a K/V tensor; member s holds seg_len_host[s] rows (its own strip's tokens).
+extern "C" int df_attn_make_kvmaps_ragged(df_comm_t comm, uint64_t tensor_off, uint64_t slot_bytes, int b,
+                                          const int32_t* seg_len_host, int heads, int d, void* maps_out, void* stream) {
   static_assert(sizeof(CUtensorMap) == DF_TENSORMAP_BYTES, "tensor map size");
   DF_REQUIRE(d % 8 == 0 && d >= 8 && d <= 192, "df_attn: head dim %d not supported (multiple of 8, <= 192)", d);
-  DF_REQUIRE(slot_bytes >= (uint64_t)b * lseg * 2 * heads * d * 2, "df_attn_make_kvmaps: slot too small");
+  DF_REQUIRE(seg_len_host != nullptr && comm.world >= 1 && comm.world <= DF_MAX_WORLD, "df_attn_make_kvmaps: bad lengths");
+  for (int s = 0; s < comm.world; ++s) {
+    DF_REQUIRE(seg_len_host[s] >= 1, "df_attn_make_kvmaps: member %d has %d K/V rows", s, seg_len_host[s]);
+    DF_REQUIRE(slot_bytes >= (uint64_t)b * seg_len_host[s] * 2 * heads * d * 2, "df_attn_make_kvmaps: slot too small");
+  }
   CUtensorMap host[DF_NBANKS * DF_MAX_WORLD];
   memset(host, 0, sizeof(host));
   const int64_t pitch = 2 * (int64_t)heads * d;
   for (int k = 0; k < DF_NBANKS; ++k)
     for (int s = 0; s < comm.world; ++s) {
       const char* base = slot_ptr(comm, comm.rank, (uint32_t)k, tensor_off, slot_bytes, s);
-      if (int rc = make_map(&host[k * comm.world + s], base, d, 2 * heads, lseg, b, pitch)) return rc;
+      if (int rc = make_map(&host[k * comm.world + s], base, d, 2 * heads, seg_len_host[s], b, pitch)) return rc;
     }
   DF_CHECK_CUDA(cudaMemcpyAsync(maps_out, host, sizeof(CUtensorMap) * DF_NBANKS * comm.world, cudaMemcpyHostToDevice,
                                 (cudaStream_t)stream));
   DF_CHECK_CUDA(cudaStreamSynchronize((cudaStream_t)stream));
   return 0;
+}
+
+extern "C" int df_attn_make_kvmaps(df_comm_t comm, uint64_t tensor_off, uint64_t slot_bytes, int b, int lseg, int heads,
+                                   int d, void* maps_out, void* stream) {
+  int32_t len[DF_MAX_WORLD];
+  for (int s = 0; s < DF_MAX_WORLD; ++s) len[s] = lseg;
+  return df_attn_make_kvmaps_ragged(comm, tensor_off, slot_bytes, b, len, heads, d, maps_out, stream);
 }
 
 namespace {
@@ -524,12 +551,10 @@ namespace {
 // Grid and work schedule of a launch (see the kernel): G resident CTAs, `a` whole units per CTA, R left-over units in P parts.
 // Policy: the left-over units of a grid that already fills the SMs are not cut -- the R CTAs of the last round have the memory
 // system to themselves, which a balanced tail would trade for partial writes and a merge -- so P > 1 only when the units leave
-// at least half of the SMs idle AND every part keeps >= 8 K/V tiles.
-void plan_schedule(int b, int lq, int lseg, int nseg, int heads, int d, bool have_ws, int& grid, Sched& sc) {
-  (void)d;
+// at least half of the SMs idle AND every part keeps >= 8 K/V tiles.  t_all: the K/V tiles of all segments together.
+void plan_schedule(int b, int lq, int t_all, int heads, bool have_ws, int& grid, Sched& sc) {
   const long long slots = sm_count();
   const long long units = (long long)((lq + BM - 1) / BM) * heads * b;
-  const int t_all = nseg * ((lseg + BN - 1) / BN);
   sc.units = (int)units;
   if (units >= slots) {
     grid = (int)slots;
@@ -553,40 +578,46 @@ size_t workspace_need(const Sched& sc, int d) {
   const size_t parts = (size_t)sc.R * sc.P;
   return WS_HEADER + 1024 + ((size_t)sc.R * sizeof(unsigned int) + 255) / 256 * 256 + parts * BM * sizeof(float2) + parts * BM * hd_pad * sizeof(float);
 }
-}  // namespace
-
-extern "C" size_t df_attn_workspace_bytes(int b, int lq, int lseg, int nseg, int heads, int d) {
-  int grid;
-  Sched sc;
-  plan_schedule(b, lq, lseg, nseg, heads, d, true, grid, sc);
-  return workspace_need(sc, d);
+// K/V tiles of all nseg segments; seg_len_host == nullptr: every segment has lseg rows
+int total_tiles(int nseg, int lseg, const int32_t* seg_len_host) {
+  int t = 0;
+  for (int s = 0; s < nseg; ++s) t += ((seg_len_host ? seg_len_host[s] : lseg) + BN - 1) / BN;
+  return t;
 }
 
-extern "C" int df_attn_fwd(df_comm_t comm, const void* q, const void* kv_own, void* out, const void* kvmaps, int b, int lq,
-                           int lseg, int heads, int d, int64_t q_pitch, int64_t kv_pitch, int64_t o_pitch, int nseg,
-                           int own_seg, const int32_t* seg_rank_host, int idx, int wait_flags, float scale, void* workspace,
-                           size_t workspace_bytes, void* stream) {
+int attn_fwd_impl(df_comm_t comm, const void* q, const void* kv_own, void* out, const void* kvmaps, int b, int lq,
+                  const int32_t* seg_len, int heads, int d, int64_t q_pitch, int64_t kv_pitch, int64_t o_pitch, int nseg,
+                  int own_seg, const int32_t* seg_rank_host, int idx, int wait_flags, float scale, void* workspace,
+                  size_t workspace_bytes, void* stream) {
   DF_REQUIRE(d % 8 == 0 && d >= 8 && d <= 192, "df_attn_fwd: head dim %d not supported (multiple of 8, <= 192)", d);
   DF_REQUIRE(nseg >= 1 && nseg <= DF_MAX_WORLD && own_seg >= 0 && own_seg < nseg, "df_attn_fwd: bad segment layout");
   DF_REQUIRE(nseg == 1 || kvmaps != nullptr, "df_attn_fwd: peer segments need tensor maps (df_attn_make_kvmaps)");
   DF_REQUIRE(q_pitch % 8 == 0 && kv_pitch % 8 == 0 && o_pitch % 8 == 0 && ((uintptr_t)q % 16) == 0 &&
                  ((uintptr_t)kv_own % 16) == 0 && ((uintptr_t)out % 16) == 0,
              "df_attn_fwd: q/kv/out must be 16-byte aligned with pitches multiple of 8");
-  DF_REQUIRE(b >= 1 && lq >= 1 && lseg >= 1 && heads >= 1 && heads <= 65535 && b <= 65535, "df_attn_fwd: bad shape");
+  DF_REQUIRE(b >= 1 && lq >= 1 && heads >= 1 && heads <= 65535 && b <= 65535, "df_attn_fwd: bad shape");
+  for (int s = 0; s < nseg; ++s) DF_REQUIRE(seg_len[s] >= 1, "df_attn_fwd: segment %d has %d K/V rows", s, seg_len[s]);
   CUtensorMap tq, tkv;
   if (int rc = make_map(&tq, q, d, heads, lq, b, q_pitch)) return rc;
-  if (int rc = make_map(&tkv, kv_own, d, 2 * heads, lseg, b, kv_pitch)) return rc;
+  if (int rc = make_map(&tkv, kv_own, d, 2 * heads, seg_len[own_seg], b, kv_pitch)) return rc;
   SegInfo segs;
+  memset(&segs, 0, sizeof(segs));
   for (int s = 0; s < DF_MAX_WORLD; ++s) segs.rank[s] = (s < nseg && seg_rank_host) ? seg_rank_host[s] : 0;
+  for (int o = 0; o < nseg; ++o) {                     // walk order: the own segment first, then the next ones cyclically
+    const int s = (own_seg + o) % nseg;
+    segs.len[o] = seg_len[s];
+    segs.tile0[o + 1] = segs.tile0[o] + (seg_len[s] + BN - 1) / BN;
+  }
+  const int t_all = segs.tile0[nseg];
   const float sc = (scale > 0.f ? scale : 1.f / sqrtf((float)d)) * 1.4426950408889634f;
   const int nblk = (d + HB - 1) / HB;
   // work schedule; the dynamic ticket counter and the K/V split of small grids need a ZERO-INITIALISED workspace of
   // df_attn_workspace_bytes() (self-resetting counters); without one every CTA walks a static list of whole units
   int grid_x;
   Sched sched;
-  plan_schedule(b, lq, lseg, nseg, heads, d, true, grid_x, sched);
+  plan_schedule(b, lq, t_all, heads, true, grid_x, sched);
   if (workspace == nullptr || workspace_bytes < workspace_need(sched, d))
-    plan_schedule(b, lq, lseg, nseg, heads, d, false, grid_x, sched);
+    plan_schedule(b, lq, t_all, heads, false, grid_x, sched);
   unsigned int* sched_ctr = sched.dyn ? (unsigned int*)workspace : nullptr;
   unsigned int* part_cnt = nullptr;
   float2* part_ml = nullptr;
@@ -609,11 +640,47 @@ extern "C" int df_attn_fwd(df_comm_t comm, const void* q, const void* kv_own, vo
       attr_set = true;                                                                                                       \
     }                                                                                                                        \
     DF_CHECK_CUDA(launch_pdl(PDL_ATTN, fmha_fwd_kernel<NB>, grid, dim3(NTHREADS), smem_bytes, (cudaStream_t)stream, tq, tkv,           \
-                             (const CUtensorMap*)kvmaps, comm, segs, (__half*)out, lq, lseg, heads, d, o_pitch, nseg,        \
+                             (const CUtensorMap*)kvmaps, comm, segs, (__half*)out, lq, heads, d, o_pitch, nseg,              \
                              own_seg, idx, wait_flags, sc, sched, part_o, part_ml, part_cnt, sched_ctr));                               \
   }
   if (nblk == 1) DF_LAUNCH_FMHA(1) else if (nblk == 2) DF_LAUNCH_FMHA(2) else DF_LAUNCH_FMHA(3)
 #undef DF_LAUNCH_FMHA
   DF_CHECK_LAUNCH();
   return 0;
+}
+}  // namespace
+
+extern "C" size_t df_attn_workspace_bytes_ragged(int b, int lq, const int32_t* seg_len_host, int nseg, int heads, int d) {
+  if (seg_len_host == nullptr || nseg < 1 || nseg > DF_MAX_WORLD) return 0;
+  int grid;
+  Sched sc;
+  plan_schedule(b, lq, total_tiles(nseg, 0, seg_len_host), heads, true, grid, sc);
+  return workspace_need(sc, d);
+}
+
+extern "C" size_t df_attn_workspace_bytes(int b, int lq, int lseg, int nseg, int heads, int d) {
+  int grid;
+  Sched sc;
+  plan_schedule(b, lq, total_tiles(nseg, lseg, nullptr), heads, true, grid, sc);
+  return workspace_need(sc, d);
+}
+
+extern "C" int df_attn_fwd_ragged(df_comm_t comm, const void* q, const void* kv_own, void* out, const void* kvmaps, int b,
+                                  int lq, const int32_t* seg_len_host, int heads, int d, int64_t q_pitch, int64_t kv_pitch,
+                                  int64_t o_pitch, int nseg, int own_seg, const int32_t* seg_rank_host, int idx, int wait_flags,
+                                  float scale, void* workspace, size_t workspace_bytes, void* stream) {
+  DF_REQUIRE(seg_len_host != nullptr, "df_attn_fwd_ragged: segment lengths missing");
+  DF_REQUIRE(nseg >= 1 && nseg <= DF_MAX_WORLD, "df_attn_fwd: bad segment layout");
+  return attn_fwd_impl(comm, q, kv_own, out, kvmaps, b, lq, seg_len_host, heads, d, q_pitch, kv_pitch, o_pitch, nseg, own_seg,
+                       seg_rank_host, idx, wait_flags, scale, workspace, workspace_bytes, stream);
+}
+
+extern "C" int df_attn_fwd(df_comm_t comm, const void* q, const void* kv_own, void* out, const void* kvmaps, int b, int lq,
+                           int lseg, int heads, int d, int64_t q_pitch, int64_t kv_pitch, int64_t o_pitch, int nseg,
+                           int own_seg, const int32_t* seg_rank_host, int idx, int wait_flags, float scale, void* workspace,
+                           size_t workspace_bytes, void* stream) {
+  int32_t len[DF_MAX_WORLD];
+  for (int s = 0; s < DF_MAX_WORLD; ++s) len[s] = lseg;
+  return attn_fwd_impl(comm, q, kv_own, out, kvmaps, b, lq, len, heads, d, q_pitch, kv_pitch, o_pitch, nseg, own_seg,
+                       seg_rank_host, idx, wait_flags, scale, workspace, workspace_bytes, stream);
 }

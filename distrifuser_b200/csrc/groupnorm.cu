@@ -69,6 +69,10 @@ struct GnExchange {   // grid barrier and cross-rank exchange of the statistics
   int mode, neg_fb, idx;
   uint64_t tensor_off, slot_bytes;
   uint32_t group_mask;
+  // statistics of source p weigh wgt[p] / sum(wgt) (its share of the patch group's rows, reduced by the gcd: equal strips give
+  // wgt = 1 and inv_w = 1/n)
+  int32_t wgt[DF_MAX_WORLD];
+  float inv_w;
 };
 
 // Fused conv-halo handling of the normalise pass (GroupNorm -> SiLU -> 3x3 conv, the ResnetBlock2D pattern): the output goes
@@ -215,23 +219,24 @@ __device__ __forceinline__ void gn_coef_sample(const GnExchange& e, int b, int G
     rd = mode == 1 ? c.clock[0] : c.clock[1];   // a synchronous exchange reads THIS epoch even inside an asynchronous step
     wait_sources(c, e.idx, e.group_mask, rd);
   }
-  const int n = __popc(e.group_mask);
   for (int g = tid; g < G; g += nthr) {
     const float2 m = mine[g];
     float mean = m.x, msq = m.y;
     if (mode != 0) {
+      // weighted sums sum_p w_p v_p (w_p = 1 on equal strips: fmaf(1, v, s) rounds exactly like s + v)
       float sx = 0.f, sy = 0.f;
       float2 own_stale = make_float2(0.f, 0.f);
       for (int p = 0; p < c.world; ++p) {
         if (!(e.group_mask >> p & 1)) continue;
         const float2 v = ((const float2*)slot_ptr(c, c.rank, rd, e.tensor_off, e.slot_bytes, p))[(size_t)b * G + g];
+        const float w = (float)e.wgt[p];
         if (p == c.rank) own_stale = v;
-        sx += v.x; sy += v.y;
+        sx = fmaf(w, v.x, sx); sy = fmaf(w, v.y, sy);
       }
-      const float invn = 1.f / (float)n;
-      if (mode == 1) { mean = sx * invn; msq = sy * invn; }
-      else if (mode == 2) { mean = sx * invn + (m.x - own_stale.x); msq = sy * invn + (m.y - own_stale.y); }
-      else { mean = (sx - own_stale.x + m.x) * invn; msq = (sy - own_stale.y + m.y) * invn; }
+      const float invw = e.inv_w, wown = (float)e.wgt[c.rank];
+      if (mode == 1) { mean = sx * invw; msq = sy * invw; }
+      else if (mode == 2) { mean = sx * invw + (m.x - own_stale.x); msq = sy * invw + (m.y - own_stale.y); }
+      else { mean = fmaf(wown, m.x, fmaf(-wown, own_stale.x, sx)) * invw; msq = fmaf(wown, m.y, fmaf(-wown, own_stale.y, sy)) * invw; }
     }
     float var = msq - mean * mean;
     if (e.neg_fb && var < 0.f) var = m.y - m.x * m.x;
@@ -436,7 +441,7 @@ namespace {
 int groupnorm_impl(df_comm_t comm, const void* x, const void* addend, int64_t addend_pitch, void* y, const void* gamma,
                    const void* beta, int b, int h, int w, int C, int groups, float eps, int mode, int bessel,
                    int neg_var_fallback, int fuse_silu, int idx, uint64_t tensor_off, uint64_t slot_bytes,
-                   uint32_t group_mask, void* scratch, void* stream, GnHalo halo) {
+                   uint32_t group_mask, const int32_t* src_weight_host, void* scratch, void* stream, GnHalo halo) {
   DF_REQUIRE(C % 8 == 0 && C % groups == 0 && C / 8 <= 512, "df_groupnorm_fwd: unsupported channel count %d", C);
   DF_REQUIRE(((uintptr_t)x % 16) == 0 && ((uintptr_t)y % 16) == 0 && ((uintptr_t)addend % 16) == 0 && addend_pitch % 8 == 0,
              "df_groupnorm_fwd: x / y / addend must be 16-byte aligned (addend pitch a multiple of 8 elements)");
@@ -460,6 +465,24 @@ int groupnorm_impl(df_comm_t comm, const void* x, const void* addend, int64_t ad
   ex.bessel = bessel ? (float)((double)ne / (double)(ne - 1)) : 1.f;
   ex.eps = eps; ex.mode = mode; ex.neg_fb = neg_var_fallback; ex.idx = idx;
   ex.tensor_off = tensor_off; ex.slot_bytes = slot_bytes; ex.group_mask = group_mask;
+  {                                                             // source weights reduced by their gcd; null = equal
+    int64_t gcd = 0, sum = 0;
+    for (int p = 0; p < DF_MAX_WORLD; ++p) {
+      ex.wgt[p] = 0;
+      if (p >= comm.world || !(group_mask >> p & 1)) continue;
+      const int64_t w = src_weight_host ? src_weight_host[p] : 1;
+      DF_REQUIRE(w >= 1, "df_groupnorm_fwd: weight %lld of source %d must be positive", (long long)w, p);
+      int64_t a = gcd, c = w;
+      while (c) { const int64_t t = a % c; a = c; c = t; }
+      gcd = a;
+    }
+    for (int p = 0; p < comm.world && p < DF_MAX_WORLD; ++p) {
+      if (!(group_mask >> p & 1)) continue;
+      ex.wgt[p] = (int32_t)((src_weight_host ? src_weight_host[p] : 1) / gcd);
+      sum += ex.wgt[p];
+    }
+    ex.inv_w = sum > 0 ? 1.f / (float)sum : 1.f;
+  }
   size_t smem = (size_t)p.lanes * C * sizeof(float2);
   {                                                             // after the fold: 2 x (red[G*tpp] + mine[G]) + coef[G]
     int tpp = p.threads / groups; if (tpp > 16) tpp = 16; if (tpp < 1) tpp = 1;
@@ -478,21 +501,32 @@ int groupnorm_impl(df_comm_t comm, const void* x, const void* addend, int64_t ad
 }
 }  // namespace
 
+extern "C" int df_groupnorm_fwd_weighted(df_comm_t comm, const void* x, const void* addend, int64_t addend_pitch, void* y,
+                                         const void* gamma, const void* beta, int b, int h, int w, int C, int groups, float eps,
+                                         int mode, int bessel, int neg_var_fallback, int fuse_silu, int idx, uint64_t tensor_off,
+                                         uint64_t slot_bytes, uint32_t group_mask, const int32_t* src_weight_host, void* scratch,
+                                         void* stream) {
+  GnHalo halo;
+  memset(&halo, 0, sizeof(halo));
+  return groupnorm_impl(comm, x, addend, addend_pitch, y, gamma, beta, b, h, w, C, groups, eps, mode, bessel, neg_var_fallback, fuse_silu, idx,
+                        tensor_off, slot_bytes, group_mask, src_weight_host, scratch, stream, halo);
+}
+
 extern "C" int df_groupnorm_fwd(df_comm_t comm, const void* x, const void* addend, int64_t addend_pitch, void* y, const void* gamma,
                                 const void* beta, int b, int h, int w, int C, int groups, float eps, int mode, int bessel,
                                 int neg_var_fallback, int fuse_silu, int idx, uint64_t tensor_off, uint64_t slot_bytes,
                                 uint32_t group_mask, void* scratch, void* stream) {
-  GnHalo halo;
-  memset(&halo, 0, sizeof(halo));
-  return groupnorm_impl(comm, x, addend, addend_pitch, y, gamma, beta, b, h, w, C, groups, eps, mode, bessel, neg_var_fallback, fuse_silu, idx,
-                        tensor_off, slot_bytes, group_mask, scratch, stream, halo);
+  return df_groupnorm_fwd_weighted(comm, x, addend, addend_pitch, y, gamma, beta, b, h, w, C, groups, eps, mode, bessel,
+                                   neg_var_fallback, fuse_silu, idx, tensor_off, slot_bytes, group_mask, nullptr, scratch, stream);
 }
 
-extern "C" int df_groupnorm_halo_fwd(df_comm_t comm, const void* x, const void* addend, int64_t addend_pitch, void* y_padded, const void* gamma,
-                                     const void* beta, int b, int h, int w, int C, int groups, float eps, int mode, int bessel,
-                                     int neg_var_fallback, int fuse_silu, int idx, uint64_t tensor_off, uint64_t slot_bytes,
-                                     uint32_t group_mask, void* scratch, int halo_idx, uint64_t halo_off,
-                                     uint64_t halo_slot_bytes, int up_rank, int down_rank, int push, int wait_flags, void* stream) {
+extern "C" int df_groupnorm_halo_fwd_weighted(df_comm_t comm, const void* x, const void* addend, int64_t addend_pitch,
+                                              void* y_padded, const void* gamma, const void* beta, int b, int h, int w, int C,
+                                              int groups, float eps, int mode, int bessel, int neg_var_fallback, int fuse_silu,
+                                              int idx, uint64_t tensor_off, uint64_t slot_bytes, uint32_t group_mask,
+                                              const int32_t* src_weight_host, void* scratch, int halo_idx, uint64_t halo_off,
+                                              uint64_t halo_slot_bytes, int up_rank, int down_rank, int push, int wait_flags,
+                                              void* stream) {
   DF_REQUIRE(halo_slot_bytes >= 2ull * b * w * C * 2, "df_groupnorm_halo_fwd: halo slot too small");
   DF_REQUIRE(up_rank < comm.world && down_rank < comm.world, "df_groupnorm_halo_fwd: neighbour outside the communicator");
   GnHalo halo;
@@ -500,5 +534,15 @@ extern "C" int df_groupnorm_halo_fwd(df_comm_t comm, const void* x, const void* 
   halo.enabled = 1; halo.h = h; halo.w = w; halo.up = up_rank; halo.down = down_rank; halo.push = push; halo.wait_flags = wait_flags;
   halo.idx = halo_idx; halo.off = halo_off; halo.slot_bytes = halo_slot_bytes; halo.c = comm;
   return groupnorm_impl(comm, x, addend, addend_pitch, y_padded, gamma, beta, b, h, w, C, groups, eps, mode, bessel, neg_var_fallback, fuse_silu,
-                        idx, tensor_off, slot_bytes, group_mask, scratch, stream, halo);
+                        idx, tensor_off, slot_bytes, group_mask, src_weight_host, scratch, stream, halo);
+}
+
+extern "C" int df_groupnorm_halo_fwd(df_comm_t comm, const void* x, const void* addend, int64_t addend_pitch, void* y_padded, const void* gamma,
+                                     const void* beta, int b, int h, int w, int C, int groups, float eps, int mode, int bessel,
+                                     int neg_var_fallback, int fuse_silu, int idx, uint64_t tensor_off, uint64_t slot_bytes,
+                                     uint32_t group_mask, void* scratch, int halo_idx, uint64_t halo_off,
+                                     uint64_t halo_slot_bytes, int up_rank, int down_rank, int push, int wait_flags, void* stream) {
+  return df_groupnorm_halo_fwd_weighted(comm, x, addend, addend_pitch, y_padded, gamma, beta, b, h, w, C, groups, eps, mode, bessel,
+                                        neg_var_fallback, fuse_silu, idx, tensor_off, slot_bytes, group_mask, nullptr, scratch,
+                                        halo_idx, halo_off, halo_slot_bytes, up_rank, down_rank, push, wait_flags, stream);
 }

@@ -16,7 +16,7 @@ from ..modules.base_module import BaseModule, nvtx_range
 from ..modules.pp.attn import DistriCrossAttentionPP, DistriSelfAttentionPP
 from ..modules.pp.conv2d import DistriConv2dPP
 from ..modules.pp.groupnorm import DistriGroupNorm
-from ..utils import DistriConfig
+from ..utils import DistriConfig, patch_rows, row_offset, split_units
 from .base_model import BaseModel
 
 
@@ -90,10 +90,38 @@ def load_static_inputs(si: dict, sample, timestep, encoder_hidden_states, added_
             si["added_cond_kwargs"][k].copy_(added_cond_kwargs[k])
 
 
+def downsample_factor(model: nn.Module) -> int:
+    """u = 2^(stride-2 downsamplers of the UNet): latent rows per row unit, so that every level holds whole rows of each unit."""
+    blocks = getattr(model, "down_blocks", None)
+    if blocks is None:
+        return 2 ** (len(model.config.block_out_channels) - 1)
+    return 2 ** sum(1 for blk in blocks if getattr(blk, "downsamplers", None) is not None)
+
+
+def row_plan(model: nn.Module, cfg: DistriConfig) -> list[int]:
+    """Units of latent rows of each patch rank (utils.split_units): rank r of n holds U // n or U // n + 1 consecutive units
+    of u rows, U = latent rows / u.  Raises ValueError for a height that cannot be split."""
+    n = cfg.n_device_per_batch
+    rows, u = cfg.height // 8, downsample_factor(model)
+    if rows % u != 0:
+        raise ValueError(f"patch parallelism needs the latent height to be a multiple of {u} (2^downsamplers of the UNet): "
+                         f"height {cfg.height} gives {rows} latent rows")
+    if rows // u < n:
+        raise ValueError(f"patch parallelism over {n} ranks needs at least {n} units of {u} latent rows: height {cfg.height} "
+                         f"gives {rows // u}")
+    return split_units(rows // u, n)
+
+
 class DistriUNetPP(BaseModel):  # for Patch Parallelism
     def __init__(self, model: nn.Module, distri_config: DistriConfig):
+        # the row plan (uneven strips when n does not divide the row units); one patch keeps the whole image, any height
+        row_units = row_plan(model, distri_config) if distri_config.n_device_per_batch > 1 else None
         install_pp_wrappers(model, distri_config)
         super().__init__(model, distri_config)
+        self.row_units = row_units
+        for module in model.modules():
+            if isinstance(module, BaseModule):
+                module.row_units = self.row_units
 
     def _step_kind(self) -> int:
         cfg = self.distri_config
@@ -163,7 +191,7 @@ class DistriUNetPP(BaseModel):  # for Patch Parallelism
                 strip = output.contiguous()
                 bs, _, hs, _ = strip.shape
                 batch0 = cfg.batch_idx() if split else 0
-                row0 = cfg.split_idx() * hs if n > 1 else 0
+                row0 = row_offset(patch_rows(self.row_units, cfg.split_idx(), hs), cfg.split_idx()) if n > 1 else 0
                 if n == 1:
                     assert hs == h
                 _lib.check(_lib.lib().df_output_gather(cm.world, strip.data_ptr(), self.output_buffer.data_ptr(), B, c, h, w,

@@ -5,7 +5,7 @@ import os
 import torch
 from torch import nn
 
-from ..utils import DistriConfig
+from ..utils import DistriConfig, patch_rows
 
 NVTX = os.environ.get("DF_NVTX", "1") != "0"     # NVTX range per wrapper call (SURVEY 5 tracing row); DF_NVTX=0 removes them
 
@@ -46,9 +46,15 @@ class BaseModule(nn.Module):
         self.counter = 0
         self.buffer_list = None
         self.idx = None
+        self.row_units = None            # units of latent rows per patch rank (DistriUNetPP's row plan); None: equal strips
 
     def forward(self, *args, **kwargs):
         raise NotImplementedError
+
+    def patch_rows(self, h: int) -> list[int]:
+        """Rows (or tokens) of every patch rank at the level where this rank holds h of them."""
+        n = self.distri_config.n_device_per_batch
+        return patch_rows(self.row_units or [1] * n, self.distri_config.split_idx(), h)
 
     def set_counter(self, counter: int = 0):
         self.counter = counter

@@ -49,37 +49,40 @@ class DistriAttentionPP(BaseModule):
         self.to_kv = to_kv
         self._kvmaps = None
 
-    def _attend(self, q, kv_own, lseg, nseg, own_seg, wait_flags, kind="self", scale=0.0, real_width=None):
-        """softmax(q k^T * scale) v over `nseg` K/V segments of `lseg` rows each; q:[b,lq,C], kv_own:[b,lseg,2C]; scale 0 =
-        1/sqrt(d) of the stored head width (pass it explicitly when the heads are zero-padded)."""
+    def _attend(self, q, kv_own, lens, own_seg, wait_flags, kind="self", scale=0.0, real_width=None):
+        """softmax(q k^T * scale) v over the K/V segments of `lens[s]` rows (the patch ranks' strips, unequal when the strips
+        are); q:[b,lq,C], kv_own:[b,lens[own_seg],2C]; scale 0 = 1/sqrt(d) of the stored head width (pass it explicitly when the
+        heads are zero-padded)."""
         attn = self.module
         b, lq, Cq = q.shape
         heads = attn.heads
         d = Cq // heads
         out = torch.empty((b, lq, Cq), dtype=q.dtype, device=q.device)
         cm = self.comm_manager
+        nseg = len(lens)
         if nseg > 1:
             comm, maps = cm.group, self._kvmaps.data_ptr()
         else:
             comm, maps = _lib.null_comm(), None
         seg_rank = (C.c_int32 * _lib.MAX_WORLD)(*range(_lib.MAX_WORLD))
+        seg_len = _lib.int32_array(lens)
         L = _lib.lib()
-        ws_bytes = L.df_attn_workspace_bytes(b, lq, lseg, nseg, heads, d)
+        ws_bytes = L.df_attn_workspace_bytes_ragged(b, lq, seg_len, nseg, heads, d)
         ws = _shared_workspace(q.device, ws_bytes).data_ptr() if ws_bytes else None
         prof = _lib.PROFILE
         if prof is not None:
             e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
             e0.record()
-        _lib.check(L.df_attn_fwd(comm, q.data_ptr(), kv_own.data_ptr(), out.data_ptr(), maps, b, lq, lseg,
-                                 heads, d, q.stride(1), kv_own.stride(1), out.stride(1), nseg, own_seg,
-                                 seg_rank, self.idx or 0, int(wait_flags), float(scale), ws, ws_bytes,
-                                 torch.cuda.current_stream().cuda_stream), "df_attn_fwd")
+        _lib.check(L.df_attn_fwd_ragged(comm, q.data_ptr(), kv_own.data_ptr(), out.data_ptr(), maps, b, lq, seg_len,
+                                        heads, d, q.stride(1), kv_own.stride(1), out.stride(1), nseg, own_seg,
+                                        seg_rank, self.idx or 0, int(wait_flags), float(scale), ws, ws_bytes,
+                                        torch.cuda.current_stream().cuda_stream), "df_attn_fwd_ragged")
         if prof is not None:
             e1.record()
             prof.append(dict(kernel="fmha_fwd_kernel", kind=kind,
-                             flops=4.0 * b * lq * nseg * lseg * (real_width or Cq),   # algorithmic: zero-padded head columns do not count
-                             bytes=2.0 * (2 * b * lq * Cq + b * nseg * lseg * 2 * Cq),
-                             shape=(b, lq, nseg * lseg, heads, d), start=e0, end=e1))
+                             flops=4.0 * b * lq * sum(lens) * (real_width or Cq),   # algorithmic: zero-padded head columns do not count
+                             bytes=2.0 * (2 * b * lq * Cq + b * sum(lens) * 2 * Cq),
+                             shape=(b, lq, sum(lens), heads, d), start=e0, end=e1))
         return out
 
     def _project_out(self, hidden_states, residual, weight=None):
@@ -114,7 +117,7 @@ class DistriCrossAttentionPP(DistriAttentionPP):
             else:
                 self.kv_cache = kv
         kv = self.kv_cache
-        out = self._attend(q, kv, kv.shape[1], 1, 0, False, kind="cross")
+        out = self._attend(q, kv, [kv.shape[1]], 0, False, kind="cross")
         out = self._project_out(out, hidden_states)
         self.counter += 1
         return out
@@ -176,8 +179,11 @@ class DistriSelfAttentionPP(DistriAttentionPP):
         d_real = c // heads
         padded = w_qkv is not None and self._head_pad != 0
         cs = heads * self._head_pad if padded else c                     # stored width of q (and of each of k, v)
+        lens = self.patch_rows(l) if n > 1 else [l]                      # tokens of every rank's strip (unequal strips differ)
         if n > 1 and self._recording() and self.idx is None:
-            self.idx = cm.register_tensor((b, l, 2 * cs), hidden_states.dtype, layer_type="attn")  # :185-190
+            # every rank's slot has the size of the LARGEST strip's K/V, so that all ranks compute the same arena layout
+            self.idx = cm.register_tensor((b, l, 2 * cs), hidden_states.dtype, layer_type="attn",                 # :185-190
+                                          slot_bytes=b * max(lens) * 2 * cs * hidden_states.element_size())
         live = n > 1 and self._bound()
         sync = live and (cfg.mode == "full_sync" or self._is_sync_step())
         ship = live and (sync or cfg.mode != "no_sync")                  # attn.py:133 / :139-140
@@ -199,16 +205,17 @@ class DistriSelfAttentionPP(DistriAttentionPP):
         sm_scale = d_real ** -0.5 if padded else 0.0
         if not live:
             # attn.py:127-131: one rank, or buffers not created yet (n identical copies of kv give the same softmax)
-            out = self._attend(q, kv, l, 1, 0, False, scale=sm_scale, real_width=c)
+            out = self._attend(q, kv, [l], 0, False, scale=sm_scale, real_width=c)
         else:
             if self._kvmaps is None:
                 self._kvmaps = torch.empty(_lib.NBANKS * n * _lib.TENSORMAP_BYTES, dtype=torch.uint8, device=q.device)
-                _lib.check(_lib.lib().df_attn_make_kvmaps(cm.group, cm.tensor_off[self.idx], cm.slot_bytes[self.idx], b, l,
-                                                          heads, cs // heads, self._kvmaps.data_ptr(),
-                                                          torch.cuda.current_stream().cuda_stream), "df_attn_make_kvmaps")
+                _lib.check(_lib.lib().df_attn_make_kvmaps_ragged(cm.group, cm.tensor_off[self.idx], cm.slot_bytes[self.idx], b,
+                                                                 _lib.int32_array(lens), heads, cs // heads,
+                                                                 self._kvmaps.data_ptr(), torch.cuda.current_stream().cuda_stream),
+                           "df_attn_make_kvmaps_ragged")
             if ship and not published:
                 cm.enqueue(self.idx, kv, async_stream=not sync)          # sync: everyone needs it this step; async: hidden
-            out = self._attend(q, kv, l, n, r, True, scale=sm_scale, real_width=c)   # attn.py:134-153, peers' segments in place
+            out = self._attend(q, kv, lens, r, True, scale=sm_scale, real_width=c)   # attn.py:134-153, peers' segments in place
         out = self._project_out(out, hidden_states, self._w_out if padded else None)
         self.counter += 1
         return out

@@ -11,7 +11,7 @@ from torch import nn
 from torch.nn import functional as F
 
 from ... import _lib, ops
-from ...utils import DistriConfig
+from ...utils import DistriConfig, patch_rows, row_offset
 from ..base_module import BaseModule, nvtx_range
 
 
@@ -30,11 +30,13 @@ class DistriConv2dPP(BaseModule):
     def sliced_forward(self, x: torch.Tensor) -> torch.Tensor:       # conv2d.py:20-41 (conv_in: 4 channels, tiny)
         cfg = self.distri_config
         b, c, h, w = x.shape
-        assert h % cfg.n_device_per_batch == 0
+        n = cfg.n_device_per_batch
+        units = self.row_units or [1] * n
         stride, padding = self.module.stride[0], self.module.padding[0]
-        out_h = h // stride // cfg.n_device_per_batch
+        assert h // stride % sum(units) == 0
         r = cfg.split_idx()
-        lo, hi = out_h * r * stride - padding, out_h * (r + 1) * stride + padding
+        rows = patch_rows(units, r, h // stride * units[r] // sum(units))      # every rank's output rows (prefix sums: uneven strips)
+        lo, hi = row_offset(rows, r) * stride - padding, row_offset(rows, r + 1) * stride + padding
         pad_t, pad_b = max(0, -lo), max(0, hi - h)
         xs = F.pad(x[:, :, max(lo, 0):min(hi, h), :], [padding, padding, pad_t, pad_b])
         return F.conv2d(xs, self.module.weight, self.module.bias, stride=stride, padding="valid")     # 4 input channels: tiny

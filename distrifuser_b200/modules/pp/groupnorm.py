@@ -70,6 +70,8 @@ class DistriGroupNorm(BaseModule):
             comm, off, sb, mask = cm.group, cm.tensor_off[self.idx], cm.slot_bytes[self.idx], cm.group_mask()
         else:
             comm, off, sb, mask = _lib.null_comm(), 0, 0, 1
+        # each rank's statistics weigh by its share of the image rows (uneven strips); the kernel reduces them by their gcd
+        weights = _lib.int32_array(self.patch_rows(h) if cfg.n_device_per_batch > 1 else [1])
         gamma = module.weight.data_ptr() if module.affine else None
         beta = module.bias.data_ptr() if module.affine else None
         prof = _lib.PROFILE
@@ -85,15 +87,17 @@ class DistriGroupNorm(BaseModule):
             assert addend.dtype == x.dtype
         st = torch.cuda.current_stream().cuda_stream
         if halo is None:
-            _lib.check(L.df_groupnorm_fwd(comm, x.data_ptr(), addend.data_ptr() if addend is not None else None, apitch, y.data_ptr(), gamma, beta, b, h, w, c, G, float(module.eps),
-                                          mode, bessel, neg_fb, int(self.fuse_silu), self.idx or 0, off, sb, mask,
-                                          self._scratch.data_ptr(), st), "df_groupnorm_fwd")
+            _lib.check(L.df_groupnorm_fwd_weighted(comm, x.data_ptr(), addend.data_ptr() if addend is not None else None, apitch,
+                                                   y.data_ptr(), gamma, beta, b, h, w, c, G, float(module.eps), mode, bessel, neg_fb,
+                                                   int(self.fuse_silu), self.idx or 0, off, sb, mask, weights,
+                                                   self._scratch.data_ptr(), st), "df_groupnorm_fwd_weighted")
         else:
             h_idx, h_off, h_sb, up, down, push = halo
-            _lib.check(L.df_groupnorm_halo_fwd(cm.group, x.data_ptr(), addend.data_ptr() if addend is not None else None, apitch, y.data_ptr(), gamma,
-                                               beta, b, h, w, c, G, float(module.eps), mode, bessel, neg_fb, int(self.fuse_silu),
-                                               self.idx or 0, off, sb, mask, self._scratch.data_ptr(), h_idx, h_off, h_sb, up, down,
-                                               int(push), 1, st), "df_groupnorm_halo_fwd")
+            _lib.check(L.df_groupnorm_halo_fwd_weighted(cm.group, x.data_ptr(), addend.data_ptr() if addend is not None else None,
+                                                        apitch, y.data_ptr(), gamma, beta, b, h, w, c, G, float(module.eps), mode,
+                                                        bessel, neg_fb, int(self.fuse_silu), self.idx or 0, off, sb, mask, weights,
+                                                        self._scratch.data_ptr(), h_idx, h_off, h_sb, up, down, int(push), 1, st),
+                       "df_groupnorm_halo_fwd_weighted")
         if prof is not None:
             e1.record()
             prof.append(dict(kernel="groupnorm", kind="gn", flops=0.0, bytes=4.0 * x.numel(), shape=tuple(x.shape),

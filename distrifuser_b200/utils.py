@@ -22,6 +22,27 @@ def is_power_of_2(n: int) -> bool:
     return (n & (n - 1) == 0) and n != 0
 
 
+# ---- row split of patch parallelism.  The latent rows form units of u = 2^(downsamplers of the UNet) rows, so that every
+#      UNet level holds a whole number of rows of each unit; patch rank r of n gets split_units(U, n)[r] consecutive units, in
+#      rank order (equal strips when n divides U).  A module that holds h rows finds every rank's rows at its own level from
+#      h alone (patch_rows): no level index is needed.
+def split_units(units: int, n: int) -> list[int]:
+    """Units of each of the n patch ranks: U // n each, and one more for the first U % n ranks."""
+    return [units // n + (1 if r < units % n else 0) for r in range(n)]
+
+
+def patch_rows(units: list[int], rank: int, h: int) -> list[int]:
+    """Rows of every patch rank at the level where rank `rank` holds h rows (also token counts: the width is common)."""
+    if any(u * h % units[rank] for u in units):
+        raise ValueError(f"{h} rows of patch rank {rank} are not a whole number of rows per unit (units {units})")
+    return [u * h // units[rank] for u in units]
+
+
+def row_offset(rows: list[int], rank: int) -> int:
+    """First row of `rank`'s strip: the prefix sum of the lower ranks' rows."""
+    return sum(rows[:rank])
+
+
 class DistriConfig:
     """Reference: distrifuser/utils.py:23-110 (arguments, derived fields, batch_idx / split_idx)."""
 

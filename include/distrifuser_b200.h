@@ -38,7 +38,7 @@ extern "C" {
 
 /* ---- errors / info ------------------------------------------------------------------------------ */
 const char* df_last_error(void);
-int df_version(void);                       /* ABI version, currently 2 */
+int df_version(void);                       /* ABI version, currently 2 (the *_ragged / *_weighted calls are additions) */
 int df_device_sm_count(int* out);
 
 /* ---- symmetric memory: replaces the flat NCCL buffers of PatchParallelismCommManager.create_buffer
@@ -113,6 +113,23 @@ int df_groupnorm_halo_fwd(df_comm_t comm, const void* x, const void* addend, int
                           int halo_idx, uint64_t halo_off, uint64_t halo_slot_bytes, int up_rank, int down_rank, int push,
                           int wait_flags, void* stream);
 
+/* Uneven row strips (patch parallelism over a latent height that the patch count does not divide into equal strips): the
+ * same two calls, with the statistics of patch-group member p weighted by src_weight_host[p] / sum of the members' weights
+ * instead of 1/n -- pass each member's row count (any positive integers; they are reduced by their gcd).  Modes, with
+ * w_p the normalised weights and m this rank's fresh moments:
+ *   1: sum_p w_p m_p (the exact moments of the whole image);  2: sum_p w_p stale_p + (m - stale_self);
+ *   3: sum_p w_p v_p with v_self = m.   src_weight_host == NULL (or equal weights) computes exactly what the calls above do. */
+int df_groupnorm_fwd_weighted(df_comm_t comm, const void* x, const void* addend, int64_t addend_pitch, void* y, const void* gamma,
+                              const void* beta, int b, int h, int w, int C, int groups, float eps, int mode, int bessel,
+                              int neg_var_fallback, int fuse_silu, int idx, uint64_t tensor_off, uint64_t slot_bytes,
+                              uint32_t group_mask, const int32_t* src_weight_host /* [comm.world] */, void* scratch, void* stream);
+int df_groupnorm_halo_fwd_weighted(df_comm_t comm, const void* x, const void* addend, int64_t addend_pitch, void* y_padded,
+                                   const void* gamma, const void* beta, int b, int h, int w, int C, int groups, float eps, int mode,
+                                   int bessel, int neg_var_fallback, int fuse_silu, int idx, uint64_t tensor_off,
+                                   uint64_t slot_bytes, uint32_t group_mask, const int32_t* src_weight_host /* [comm.world] */,
+                                   void* scratch, int halo_idx, uint64_t halo_off, uint64_t halo_slot_bytes, int up_rank,
+                                   int down_rank, int push, int wait_flags, void* stream);
+
 /* ---- conv halo exchange: replaces the boundary stack + all_gather + cat/pad of DistriConv2dPP.forward
  *      (distrifuser/modules/pp/conv2d.py:72-93).  x: [b,h,w,C] NHWC fp16, one halo row (padding 1).
  *      df_halo_push sends x's first row to patch-neighbour `up_rank` (its bottom halo) and x's last row to
@@ -147,6 +164,20 @@ int df_attn_fwd(df_comm_t comm, const void* q, const void* kv_own, void* out, co
                 int b, int lq, int lseg, int heads, int d, int64_t q_pitch, int64_t kv_pitch, int64_t o_pitch,
                 int nseg, int own_seg, const int32_t* seg_rank_host, int idx, int wait_flags, float scale,
                 void* workspace, size_t workspace_bytes, void* stream);
+/* Segments of unequal length (uneven row strips): the same three calls with per-segment K/V row counts instead of one lseg.
+ *   df_attn_make_kvmaps_ragged: seg_len_host[s] = rows held by communicator member s (its slot stores [b, len_s, 2*heads*d]);
+ *                               slot_bytes must hold the longest.
+ *   df_attn_workspace_bytes_ragged / df_attn_fwd_ragged: seg_len_host[s] = rows of segment s (s < nseg); the own segment is
+ *                               kv_own with seg_len_host[own_seg] rows.  K/V is the concatenation of the segments; each
+ *                               segment's last tile is masked at its own length, and the split schedule cuts the total tile
+ *                               count.  Equal lengths compute exactly what the calls above compute (same launch). */
+int df_attn_make_kvmaps_ragged(df_comm_t comm, uint64_t tensor_off, uint64_t slot_bytes, int b, const int32_t* seg_len_host,
+                               int heads, int d, void* maps_out /* device, DF_NBANKS*world*DF_TENSORMAP_BYTES */, void* stream);
+size_t df_attn_workspace_bytes_ragged(int b, int lq, const int32_t* seg_len_host, int nseg, int heads, int d);
+int df_attn_fwd_ragged(df_comm_t comm, const void* q, const void* kv_own, void* out, const void* kvmaps,
+                       int b, int lq, const int32_t* seg_len_host, int heads, int d, int64_t q_pitch, int64_t kv_pitch,
+                       int64_t o_pitch, int nseg, int own_seg, const int32_t* seg_rank_host, int idx, int wait_flags, float scale,
+                       void* workspace, size_t workspace_bytes, void* stream);
 
 /* ---- final epsilon gather: replaces the blocking world all_gather + cat(dim=2) at the end of
  *      DistriUNetPP.forward (distrifuser/models/distri_sdxl_unet_pp.py:162-169,186-193).
