@@ -1,4 +1,5 @@
-"""Reference: distrifuser/models/base_model.py:8-52 (same attributes and methods).
+"""Reference: distrifuser/models/base_model.py:8-52 (same attributes and methods), plus the per-call protocol that
+DistriUNetPP and NaivePatchUNet share (distri_sdxl_unet_pp.py:42-214 / naive_patch_sdxl.py:27-219).
 
 The reference derives BaseModel from diffusers' (ModelMixin, ConfigMixin): StableDiffusion(XL)Pipeline.from_pretrained(...,
 unet=DistriUNetPP) type-checks the component against ModelMixin.  When diffusers is importable the same bases are used
@@ -6,7 +7,8 @@ here; without it (this image) a plain nn.Module carries the `dtype` / `device` p
 import torch
 from torch import nn
 
-from ..modules.base_module import BaseModule
+from .. import _lib
+from ..modules.base_module import BaseModule, nvtx_range
 from ..utils import DistriConfig, PatchParallelismCommManager
 
 try:  # pragma: no cover - depends on the environment
@@ -16,7 +18,44 @@ except Exception:
     _BASES = (nn.Module,)
 
 
+def _output_cls():
+    try:
+        from diffusers.models.unet_2d_condition import UNet2DConditionOutput
+    except Exception:
+        from ..compat.unet_2d_condition import UNet2DConditionOutput
+    return UNet2DConditionOutput
+
+
+def cfg_branch(cfg: DistriConfig, sample, timestep, encoder_hidden_states, added_cond_kwargs):
+    """This rank's half of the CFG batch (distri_sdxl_unet_pp.py:77-87 / 134-146)."""
+    i = cfg.batch_idx()
+    sample = sample[i:i + 1]
+    if torch.is_tensor(timestep) and timestep.ndim > 0:
+        timestep = timestep[i:i + 1]
+    encoder_hidden_states = encoder_hidden_states[i:i + 1]
+    if added_cond_kwargs is not None:                                # new dict: the caller's is not mutated (SURVEY D-10)
+        added_cond_kwargs = {k: v[i:i + 1] for k, v in added_cond_kwargs.items()}
+    return sample, timestep, encoder_hidden_states, added_cond_kwargs
+
+
+def load_static_inputs(si: dict, sample, timestep, encoder_hidden_states, added_cond_kwargs) -> None:
+    """Copies a call's inputs into the captured graphs' static inputs (distri_sdxl_unet_pp.py:89-106)."""
+    assert si["sample"].shape == sample.shape
+    si["sample"].copy_(sample)
+    if torch.is_tensor(timestep):
+        si["timestep"].copy_(timestep.expand(si["timestep"].shape) if timestep.ndim == 0 else timestep)
+    else:
+        si["timestep"].fill_(timestep)                               # no .item() host sync (SURVEY A6)
+    si["encoder_hidden_states"].copy_(encoder_hidden_states)
+    if added_cond_kwargs is not None:
+        for k in added_cond_kwargs:
+            si["added_cond_kwargs"][k].copy_(added_cond_kwargs[k])
+
+
 class BaseModel(*_BASES):
+    """A wrapper supplies what differs between the parallelisms: `_strip` (the UNet input of this rank and where its output
+    lands in the image), `_step_kind`, `_graph_idx`, and the counters the pipeline pre-runs and captures."""
+
     def __init__(self, model: nn.Module, distri_config: DistriConfig):
         super(BaseModel, self).__init__()
         self.model = model
@@ -31,8 +70,112 @@ class BaseModel(*_BASES):
         self.cuda_graphs = None
         self.graph_launches = None       # number of this package's kernels inside each captured graph
 
-    def forward(self, *args, **kwargs):
+    def _strip(self, sample):
+        """-> (UNet input of this rank, (row0, col0, hs, ws): the rows and columns of the image its output covers)."""
         raise NotImplementedError
+
+    def _step_kind(self) -> int:
+        """df_step_begin kind of the current counter: 0 = synchronous, 1 = asynchronous, 2 = frozen."""
+        raise NotImplementedError
+
+    def _graph_idx(self) -> int:
+        """Captured graph that serves the current counter (an index into graph_counters())."""
+        raise NotImplementedError
+
+    def prerun_counters(self) -> list[int]:
+        """Counters the pipeline runs eagerly before capturing, so that library autotuning and scratch allocations happen
+        outside the capture."""
+        raise NotImplementedError
+
+    def graph_counters(self) -> list[int]:
+        """Counters at which the pipeline captures one CUDA graph each."""
+        raise NotImplementedError
+
+    @nvtx_range()
+    def forward(
+        self,
+        sample: torch.FloatTensor,
+        timestep,
+        encoder_hidden_states: torch.Tensor,
+        class_labels=None,
+        timestep_cond=None,
+        attention_mask=None,
+        cross_attention_kwargs=None,
+        added_cond_kwargs=None,
+        down_block_additional_residuals=None,
+        mid_block_additional_residual=None,
+        down_intrablock_additional_residuals=None,
+        encoder_attention_mask=None,
+        return_dict: bool = True,
+        record: bool = False,
+    ):
+        cfg = self.distri_config
+        b, c, h, w = sample.shape
+        assert (class_labels is None and timestep_cond is None and attention_mask is None
+                and cross_attention_kwargs is None and down_block_additional_residuals is None
+                and mid_block_additional_residual is None and down_intrablock_additional_residuals is None
+                and encoder_attention_mask is None)                  # distri_sdxl_unet_pp.py:63-72
+        split = cfg.world_size > 1 and cfg.do_classifier_free_guidance and cfg.split_batch
+        if split:
+            assert b == 2
+            sample, timestep, encoder_hidden_states, added_cond_kwargs = cfg_branch(
+                cfg, sample, timestep, encoder_hidden_states, added_cond_kwargs)
+        B = 2 if split else b
+
+        if cfg.use_cuda_graph and not record and self.cuda_graphs is not None:
+            load_static_inputs(self.static_inputs, sample, timestep, encoder_hidden_states, added_cond_kwargs)
+            graph_idx = self._graph_idx()                            # distri_sdxl_unet_pp.py:108-113
+            self.cuda_graphs[graph_idx].replay()
+            if self.graph_launches is not None:
+                _lib.LAUNCHES["total"] += self.graph_launches[graph_idx]
+            output = self.static_outputs[graph_idx]
+        else:
+            cm = self.comm_manager
+            live = cm is not None and cm.arena is not None
+            if cm is not None and cm.arena is None and cfg.world_size > 1 and cm.output_spec is None:
+                cm.register_output(B, c, h, w)
+            if live:
+                cm.step_begin(self._step_kind())
+            # NHWC inside the UNet; `sample` itself stays the (sliced) view of the caller's tensor so that a captured
+            # graph re-reads the static input on every replay
+            x, (row0, col0, hs, ws) = self._strip(sample)
+            output = self.model(x.contiguous(memory_format=torch.channels_last), timestep, encoder_hidden_states,
+                                added_cond_kwargs=added_cond_kwargs, return_dict=False)[0]
+            if cfg.world_size > 1 and live:                          # distri_sdxl_unet_pp.py:162-169 / 186-193
+                # Every rank waits here for the strips of every world rank: the gather is a per-call world barrier, which
+                # is what keeps the output banks safe to reuse (BANK-REUSE INVARIANT in utils.py).
+                if self.output_buffer is None:
+                    self.output_buffer = torch.empty((B, c, h, w), device=output.device, dtype=output.dtype)
+                strip = output.contiguous()
+                bs = strip.shape[0]
+                assert tuple(strip.shape) == (bs, c, hs, ws)
+                batch0 = cfg.batch_idx() if split else 0
+                _lib.check(_lib.lib().df_output_gather_2d(cm.world, strip.data_ptr(), self.output_buffer.data_ptr(),
+                                                          B, c, h, w, bs, hs, ws, batch0, row0, col0, 0, cm.output_off,
+                                                          torch.cuda.current_stream().cuda_stream), "df_output_gather_2d")
+                output = self.output_buffer
+            elif cfg.world_size > 1:
+                # registration pass: buffers do not exist yet, the value is never consumed
+                output = output.new_zeros((B, c, h, w))
+            if cm is not None:
+                cm.join()
+            if record:
+                if self.static_inputs is None:                       # distri_sdxl_unet_pp.py:194-201
+                    self.static_inputs = {"sample": sample, "timestep": timestep,
+                                          "encoder_hidden_states": encoder_hidden_states,
+                                          "added_cond_kwargs": added_cond_kwargs}
+                self.synchronize()
+
+        if return_dict:
+            output = _output_cls()(sample=output)
+        else:
+            output = (output,)
+        self.counter += 1
+        return output
+
+    @property
+    def add_embedding(self):
+        return self.model.add_embedding
 
     def set_counter(self, counter: int = 0):                        # base_model.py:27-31
         self.counter = counter

@@ -13,9 +13,9 @@ NVTX = os.environ.get("DF_NVTX", "1") != "0"     # NVTX range per wrapper call (
 _HAS_CUDA = None
 
 
-def nvtx_range(name: str):
-    """Decorator: brackets a wrapper's forward with an NVTX range `name[idx]` when CUDA is in use (shows up in nsys / ncu
-    --nvtx; a no-op on captured-graph replays, where Python does not run)."""
+def nvtx_range(name: str | None = None):
+    """Decorator: brackets a wrapper's forward with an NVTX range `name[idx]` (default name: the class of `self`) when CUDA is
+    in use (shows up in nsys / ncu --nvtx; a no-op on captured-graph replays, where Python does not run)."""
     def deco(fn):
         if not NVTX:
             return fn
@@ -27,8 +27,8 @@ def nvtx_range(name: str):
                 _HAS_CUDA = torch.cuda.is_available()
             if not _HAS_CUDA:
                 return fn(self, *args, **kwargs)
-            idx = getattr(self, "idx", None)
-            torch.cuda.nvtx.range_push(name if idx is None else f"{name}[{idx}]")
+            label, idx = name or type(self).__name__, getattr(self, "idx", None)
+            torch.cuda.nvtx.range_push(label if idx is None else f"{label}[{idx}]")
             try:
                 return fn(self, *args, **kwargs)
             finally:

@@ -69,9 +69,7 @@ class _DistriPipelineBase:
             unet.set_counter(0)
             unet(**static_inputs, return_dict=False, record=True)    # registration pass (pipelines.py:138-139)
             comm_manager.create_buffer()                             # pipelines.py:140-141
-        # pre-run (pipelines.py:144-145); naive patch also runs the column strip of its second graph eagerly, so that library
-        # autotuning and the wrappers' scratch allocations happen outside the capture
-        for counter in ([0, 1] if cfg.parallelism == "naive_patch" and cfg.split_scheme == "alternate" else [0]):
+        for counter in unet.prerun_counters():                      # pre-run (pipelines.py:144-145)
             unet.set_counter(counter)
             unet(**static_inputs, return_dict=False, record=True)
         self.static_inputs = static_inputs
@@ -80,8 +78,7 @@ class _DistriPipelineBase:
 
     @torch.no_grad()
     def _capture_graphs(self):
-        """Patch parallelism: three graphs, synchronous step, first asynchronous step, steady state.  Naive patch: the graphs
-        of counters 0 and 1, the row and column strips of `alternate` (pipelines.py:147-165)."""
+        """One graph per counter of unet.graph_counters() (pipelines.py:147-165)."""
         cfg, unet, static_inputs = self.distri_config, self.pipeline.unet, self.static_inputs
         static_outputs, cuda_graphs = [], []
         unet.setup_cuda_graph(None, None, None)
@@ -89,10 +86,6 @@ class _DistriPipelineBase:
             if self.comm_manager is not None:
                 self.comm_manager.clear()
             torch.cuda.synchronize()
-            if cfg.parallelism == "naive_patch":
-                counters = [0, 1]
-            else:
-                counters = [0, cfg.warmup_steps + 1, cfg.warmup_steps + 2]
             unet.static_inputs = None
             pool = None
             from . import _lib
@@ -105,7 +98,7 @@ class _DistriPipelineBase:
             patch_peers = cfg.parallelism == "patch" and cfg.n_device_per_batch > 1
             prio = int(os.environ.get("DF_COMPUTE_PRIO", "-1" if patch_peers else "0"))
             capture_stream = torch.cuda.Stream(device=cfg.device, priority=prio)
-            for counter in counters:
+            for counter in unet.graph_counters():
                 graph = torch.cuda.CUDAGraph()
                 n0 = _lib.LAUNCHES["total"]
                 with torch.cuda.graph(graph, pool=pool, stream=capture_stream):

@@ -329,12 +329,12 @@ class PatchParallelismCommManager:
 
     # ------------------------------------------------------------------ step protocol
     # BANK-REUSE INVARIANT.  Bank e % 3 is overwritten by the peers' stores of epoch e+3 without any "consumed"
-    # acknowledgement.  That is safe only because every UNet call ends with df_output_gather, which makes each rank wait
+    # acknowledgement.  That is safe only because every UNet call ends with df_output_gather_2d, which makes each rank wait
     # for the epsilon strip of EVERY world rank: no rank can start call t+1 before all ranks finished the kernels of call
     # t, so ranks drift by < 1 call and a store of epoch e+3 can never meet a read of epoch e (reads of epoch e happen in
-    # calls e and e+1 only).  NaivePatchUNet ends every call with the same world gather (df_output_gather_2d), so its output
-    # banks obey the same bound.  A path that skips the gather (e.g. returning the local strip) must add its own per-call
-    # world barrier, or stale K/V / halo rows get corrupted silently.
+    # calls e and e+1 only).  BaseModel.forward makes that gather for DistriUNetPP and NaivePatchUNet alike.  A path that
+    # skips the gather (e.g. returning the local strip) must add its own per-call world barrier, or stale K/V / halo rows
+    # get corrupted silently.
     def step_begin(self, kind: int):
         """kind 0 = synchronous, 1 = asynchronous, 2 = frozen (see df_step_begin)."""
         st = torch.cuda.current_stream().cuda_stream

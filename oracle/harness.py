@@ -3,6 +3,8 @@
 `impl="oracle"`    runs the restatement in oracle/pp_modules.py (works anywhere).
 `impl="reference"` runs the UNMODIFIED reference modules imported from /root/reference through the
                    diffusers stub (only possible in the build container; used by oracle/make_golden.py).
+The UNet drivers serve every UNet case type: patch parallelism on equal (UNetCase) or uneven (RaggedCase) row strips, and
+naive patch (naive_patch.NaiveCase); the case's config_kwargs() choose the wrapper.
 Both follow the reference's own bring-up order (pipelines.py:131-145): registration pass, create buffers,
 pre-run pass, then `set_counter(0)` and the denoising calls (pipelines.py:57).
 """
@@ -150,31 +152,47 @@ def run_chain(case, impl="oracle"):
 
 
 # ---------------------------------------------------------------------------------------------- UNet
-def _unet_worker(rank, case, impl, port, outdir):
+def _unet_config(case, rank):
+    """DuckConfig of a UNet case (patch, naive patch or uneven strips) on `rank`, its batch groups made."""
+    from oracle import workloads as W
+    cfg = W.DuckConfig(case.world_size, rank, **case.config_kwargs())
+    if case.world_size > 1:
+        _groups(cfg)
+    return cfg
+
+
+def _oracle_unet(unet, cfg, bessel=True):
+    from oracle import pp_modules as P
+    if cfg.parallelism == "naive_patch":
+        from oracle.naive_patch import OracleNaivePatchUNet
+        return OracleNaivePatchUNet(unet, cfg)
+    return P.OracleUNetPP(unet, cfg, bessel=bessel)
+
+
+def _unet_worker(rank, case, impl, bessel, row_units, port, outdir):
     _paths(impl)
     from oracle import workloads as W
     _init(rank, case.world_size, port)
-    cfg = W.DuckConfig(case.world_size, rank, height=8 * case.latent, width=8 * case.latent,
-                       do_classifier_free_guidance=case.cfg, split_batch=case.split_batch,
-                       warmup_steps=case.warmup_steps, comm_checkpoint=case.comm_checkpoint, mode=case.mode)
-    if case.world_size > 1:
-        _groups(cfg)
+    cfg = _unet_config(case, rank)
     ucfg = W.unet_config(case.family)
     unet = W.make_unet(case.family, case.weight_seed)
     first = W.unet_inputs(case, 0, ucfg)
     outs = []
     with torch.no_grad():
         if impl == "reference":
-            from distrifuser.models.distri_sdxl_unet_pp import DistriUNetPP
             from distrifuser.utils import PatchParallelismCommManager
-            model = DistriUNetPP(unet, cfg)
+            if cfg.parallelism == "naive_patch":
+                from distrifuser.models.naive_patch_sdxl import NaivePatchUNet as Model
+            else:
+                from distrifuser.models.distri_sdxl_unet_pp import DistriUNetPP as Model
+            model = Model(unet, cfg)
             comm = None
             if cfg.n_device_per_batch > 1:                                   # pipelines.py:131-141
                 comm = PatchParallelismCommManager(cfg)
                 model.set_comm_manager(comm)
                 model.set_counter(0)
                 model(**first, return_dict=False, record=True)
-                if comm.numel > 0:
+                if comm.numel > 0:                                            # naive patch registers nothing
                     comm.create_buffer()
             model.set_counter(0)
             model(**first, return_dict=False, record=True)                    # pipelines.py:144-145
@@ -184,8 +202,9 @@ def _unet_worker(rank, case, impl, port, outdir):
             if comm is not None:
                 comm.clear()
         else:
-            from oracle import pp_modules as P
-            model = P.OracleUNetPP(unet, cfg)
+            model = _oracle_unet(unet, cfg, bessel)
+            if row_units is not None:
+                assert model.units == row_units, f"oracle row plan {model.units}, expected {row_units}"
             model.prepare(first)
             model.set_counter(0)
             for t in range(case.steps):
@@ -196,14 +215,21 @@ def _unet_worker(rank, case, impl, port, outdir):
         dist.destroy_process_group()
 
 
-def run_unet(case, impl="oracle"):
-    """-> outs[step] = eps prediction [B,4,S,S] (asserted identical on every rank)."""
+def run_ranks(worker, case, *args):
+    """Runs worker(rank, case, *args, port, outdir) on every rank -> what each rank saved."""
     with tempfile.TemporaryDirectory() as d:
         if case.world_size == 1:
-            _unet_worker(0, case, impl, 0, d)
+            worker(0, case, *args, 0, d)
         else:
-            mp.spawn(_unet_worker, args=(case, impl, free_port(), d), nprocs=case.world_size, join=True)
-        per_rank = [torch.load(os.path.join(d, f"rank{r}.pt")) for r in range(case.world_size)]
+            mp.spawn(worker, args=(case, *args, free_port(), d), nprocs=case.world_size, join=True)
+        return [torch.load(os.path.join(d, f"rank{r}.pt")) for r in range(case.world_size)]
+
+
+def run_unet(case, impl="oracle", bessel=True, row_units=None):
+    """-> outs[step] = eps prediction [B,4,H,W] (asserted identical on every rank).  The case picks the UNet wrapper: patch
+    parallelism (UNetCase, RaggedCase) or naive patch (NaiveCase).  `bessel=False` drops the oracle GroupNorm's local-count
+    Bessel factor; `row_units`, when given, is asserted to be the oracle's row plan."""
+    per_rank = run_ranks(_unet_worker, case, impl, bessel, row_units)
     for r in range(1, case.world_size):
         for a, b in zip(per_rank[0], per_rank[r]):
             assert torch.equal(a, b), "final output must be identical on all ranks (distri_sdxl_unet_pp.py:166-168)"
@@ -212,7 +238,7 @@ def run_unet(case, impl="oracle"):
 
 # ---------------------------------------------------------------------------------------------- denoising trajectory
 class _OracleUNetAdapter:
-    """Gives OracleUNetPP the call signature the latent pipeline uses (unet(x, t, encoder_hidden_states=..., ...)[0])."""
+    """Gives an oracle UNet wrapper the call signature the latent pipeline uses (unet(x, t, encoder_hidden_states=...)[0])."""
 
     def __init__(self, model, config):
         self.model, self.config = model, config
@@ -227,27 +253,22 @@ class _OracleUNetAdapter:
         return (self.model(sample, t, encoder_hidden_states, added_cond_kwargs=added_cond_kwargs),)
 
 
-def _traj_worker(rank, case, port, outdir, num_steps, guidance):
+def _traj_worker(rank, case, num_steps, guidance, port, outdir):
     _paths("oracle")
-    from oracle import pp_modules as P
     from oracle import workloads as W
     from distrifuser_b200.compat.pipeline import SyntheticLatentPipeline      # the denoising loop itself is shared code:
     _init(rank, case.world_size, port)                                       # only the UNet path differs between the arms
-    cfg = W.DuckConfig(case.world_size, rank, height=8 * case.latent, width=8 * case.latent,
-                       do_classifier_free_guidance=case.cfg, split_batch=case.split_batch,
-                       warmup_steps=case.warmup_steps, comm_checkpoint=case.comm_checkpoint, mode=case.mode)
-    if case.world_size > 1:
-        _groups(cfg)
+    cfg = _unet_config(case, rank)
     ucfg = W.unet_config(case.family)
     unet = W.make_unet(case.family, case.weight_seed)
-    model = P.OracleUNetPP(unet, cfg)
+    model = _oracle_unet(unet, cfg)
     model.prepare(W.unet_inputs(case, 0, ucfg))
     pipe = SyntheticLatentPipeline(_OracleUNetAdapter(model, unet.config), sdxl=ucfg.get("addition_embed_type") == "text_time",
                                    device="cpu", dtype=torch.float32)
     model.set_counter(0)
     g = torch.Generator().manual_seed(case.input_seed)
     with torch.no_grad():
-        lat = pipe(prompt="a photo", height=8 * case.latent, width=8 * case.latent, num_inference_steps=num_steps,
+        lat = pipe(prompt="a photo", height=cfg.height, width=cfg.width, num_inference_steps=num_steps,
                    guidance_scale=guidance, generator=g).images
     torch.save(lat, os.path.join(outdir, f"rank{rank}.pt"))
     if case.world_size > 1:
@@ -256,13 +277,8 @@ def _traj_worker(rank, case, port, outdir, num_steps, guidance):
 
 
 def run_trajectory(case, num_steps=8, guidance=5.0):
-    """Final latents of a `num_steps` Euler trajectory with the ORACLE UNet path (fp32 CPU) -> [1,4,S,S]."""
-    with tempfile.TemporaryDirectory() as d:
-        if case.world_size == 1:
-            _traj_worker(0, case, 0, d, num_steps, guidance)
-        else:
-            mp.spawn(_traj_worker, args=(case, free_port(), d, num_steps, guidance), nprocs=case.world_size, join=True)
-        outs = [torch.load(os.path.join(d, f"rank{r}.pt")) for r in range(case.world_size)]
+    """Final latents of a `num_steps` Euler trajectory with the ORACLE UNet path (fp32 CPU) -> [1,4,H,W]."""
+    outs = run_ranks(_traj_worker, case, num_steps, guidance)
     for o in outs[1:]:
         assert torch.equal(o, outs[0])
     return outs[0]

@@ -1,9 +1,9 @@
 """TEST INFRASTRUCTURE (oracle).  Generates tests/golden/*.pt by EXECUTING THE UNMODIFIED REFERENCE
-(/root/reference/distrifuser/modules/pp/*.py, models/distri_sdxl_unet_pp.py, utils.py:112-199) on CPU under
-gloo, through the diffusers stub.  Runs only in the build container (the reference tree does not exist on
-the GPU box); the vectors it writes are committed.
+(/root/reference/distrifuser/modules/pp/*.py, models/distri_sdxl_unet_pp.py, models/naive_patch_sdxl.py,
+utils.py:112-199) on CPU under gloo, through the diffusers stub.  Runs only in the build container (the reference
+tree does not exist on the GPU box); the vectors it writes are committed.
 
-    python -m oracle.make_golden [--only chain|unet] [--case NAME]
+    python -m oracle.make_golden [--only chain|unet|naive] [--case NAME]
 """
 import argparse
 import os
@@ -16,14 +16,14 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "oracle", "diffusers_stub"))
 
-from oracle import harness, workloads  # noqa: E402
+from oracle import harness, naive_patch, workloads  # noqa: E402
 
 GOLDEN = os.path.join(ROOT, "tests", "golden")
 
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--only", choices=["chain", "unet"], default=None)
+    ap.add_argument("--only", choices=["chain", "unet", "naive"], default=None)
     ap.add_argument("--case", default=None)
     a = ap.parse_args()
     os.makedirs(GOLDEN, exist_ok=True)
@@ -52,6 +52,16 @@ def main():
                         "source": "reference DistriUNetPP @ /root/reference over oracle/diffusers_stub, gloo, fp32"},
                        os.path.join(GOLDEN, f"unet_{case.name}.pt"))
             print(f"unet_{case.name}: {time.time() - t0:.1f}s  std={outs[-1].std():.4f}", flush=True)
+    if a.only in (None, "naive"):
+        for case in naive_patch.NAIVE_CASES:
+            if a.case and case.name != a.case:
+                continue
+            t0 = time.time()
+            outs = harness.run_unet(case, impl="reference")
+            torch.save({"case": case.__dict__, "outs": [o.clone() for o in outs],
+                        "source": "reference NaivePatchUNet @ /root/reference over oracle/diffusers_stub, gloo, fp32"},
+                       os.path.join(GOLDEN, f"{case.name}.pt"))
+            print(f"{case.name}: {time.time() - t0:.1f}s  std={outs[-1].std():.4f}", flush=True)
 
 
 if __name__ == "__main__":

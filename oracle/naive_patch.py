@@ -1,31 +1,25 @@
 """TEST INFRASTRUCTURE (oracle) -- the naive patch baseline (parallelism="naive_patch").
 
 `OracleNaivePatchUNet` restates distrifuser/models/naive_patch_sdxl.py on CPU in fp32: slice this rank's CFG half and
-strip -> plain UNet -> gloo all_gather -> cat.  `run_naive_unet` drives it (impl="oracle") or the UNMODIFIED reference
-NaivePatchUNet (impl="reference", through the diffusers stub; only where the reference tree exists) in the reference's
-bring-up order, as harness.run_unet does for DistriUNetPP.  `run_naive_trajectory` is the denoising-loop counterpart of
-harness.run_trajectory.  Running this module writes the naive-patch golden vectors from the reference:
-
-    python -m oracle.naive_patch [--case NAME]
+strip -> plain UNet -> gloo all_gather -> cat.  oracle/harness.py drives it (impl="oracle"), or the UNMODIFIED reference
+NaivePatchUNet (impl="reference"), for a NaiveCase: `run_naive_unet` / `run_naive_trajectory` are harness.run_unet /
+harness.run_trajectory under the names the naive-patch tests use.  `python -m oracle.make_golden --only naive` writes the
+naive-patch golden vectors from the reference.
 """
 from __future__ import annotations
 
-import argparse
 import dataclasses
-import os
-import tempfile
-import time
 
 import torch
 from torch import distributed as dist
-from torch import multiprocessing as mp
 
-from oracle import harness
+from oracle.harness import run_trajectory as run_naive_trajectory  # noqa: F401
+from oracle.harness import run_unet as run_naive_unet  # noqa: F401
 
 
 @dataclasses.dataclass(frozen=True)
 class NaiveCase:
-    """One naive-patch parity case (duck-types the fields of UNetCase that workloads.unet_inputs reads)."""
+    """One naive-patch parity case (the drivers read it through `batch`, `hw` and `config_kwargs()`, as for UNetCase)."""
     name: str
     family: str = "tiny_sdxl"        # tiny_sdxl | tiny_sd15
     world_size: int = 2
@@ -41,6 +35,14 @@ class NaiveCase:
     def batch(self):
         return 2 if self.cfg else 1
 
+    @property
+    def hw(self):
+        return self.latent, self.latent
+
+    def config_kwargs(self) -> dict:
+        return dict(height=8 * self.latent, width=8 * self.latent, do_classifier_free_guidance=self.cfg,
+                    split_batch=self.split_batch, parallelism="naive_patch", split_scheme=self.scheme)
+
 
 NAIVE_CASES = (
     NaiveCase("naive_sdxl_w2_row", world_size=2, scheme="row"),                          # n=2, b=2
@@ -50,14 +52,6 @@ NAIVE_CASES = (
     NaiveCase("naive_sd15_w4_col", family="tiny_sd15", world_size=4, scheme="col"),      # n=4, SD1.x topology
     NaiveCase("naive_sdxl_w8_split_col", world_size=8, split_batch=True, scheme="col"),  # n=4, b=1
 )
-
-
-def naive_config(case, rank: int):
-    from oracle import workloads as W
-    cfg = W.DuckConfig(case.world_size, rank, height=8 * case.latent, width=8 * case.latent,
-                       do_classifier_free_guidance=case.cfg, split_batch=case.split_batch)
-    cfg.parallelism, cfg.split_scheme = "naive_patch", case.scheme
-    return cfg
 
 
 class OracleNaivePatchUNet:
@@ -70,6 +64,9 @@ class OracleNaivePatchUNet:
 
     def set_counter(self, c: int = 0):
         self.counter = c
+
+    def prepare(self, inputs):
+        """Nothing to size or pre-run: naive patch registers no buffers."""
 
     def split_dim(self) -> int:
         return {"row": 2, "col": 3, "alternate": 2 if self.counter % 2 == 0 else 3}[self.cfg.split_scheme]
@@ -96,112 +93,3 @@ class OracleNaivePatchUNet:
         if split:
             return torch.cat([torch.cat(parts[:n], dim), torch.cat(parts[n:], dim)], 0)
         return torch.cat(parts, dim)
-
-
-def _naive_worker(rank, case, impl, port, outdir):
-    harness._paths(impl)
-    from oracle import workloads as W
-    harness._init(rank, case.world_size, port)
-    cfg = naive_config(case, rank)
-    if case.world_size > 1:
-        harness._groups(cfg)
-    ucfg = W.unet_config(case.family)
-    unet = W.make_unet(case.family, case.weight_seed)
-    first = W.unet_inputs(case, 0, ucfg)
-    outs = []
-    with torch.no_grad():
-        if impl == "reference":
-            from distrifuser.models.naive_patch_sdxl import NaivePatchUNet
-            from distrifuser.utils import PatchParallelismCommManager
-            model = NaivePatchUNet(unet, cfg)
-            if cfg.n_device_per_batch > 1:                                   # pipelines.py:131-141 (nothing registers)
-                model.set_comm_manager(PatchParallelismCommManager(cfg))
-                model.set_counter(0)
-                model(**first, return_dict=False, record=True)
-            model.set_counter(0)
-            model(**first, return_dict=False, record=True)                    # pipelines.py:144-145
-            model.set_counter(0)                                              # pipelines.py:57
-            for t in range(case.steps):
-                outs.append(model(**W.unet_inputs(case, t, ucfg), return_dict=False)[0].clone())
-        else:
-            model = OracleNaivePatchUNet(unet, cfg)
-            model.set_counter(0)
-            for t in range(case.steps):
-                outs.append(model(**W.unet_inputs(case, t, ucfg)).clone())
-    torch.save(outs, os.path.join(outdir, f"rank{rank}.pt"))
-    if case.world_size > 1:
-        dist.barrier()
-        dist.destroy_process_group()
-
-
-def run_naive_unet(case, impl="oracle"):
-    """-> outs[step] = eps prediction [B,4,S,S] (asserted identical on every rank)."""
-    with tempfile.TemporaryDirectory() as d:
-        if case.world_size == 1:
-            _naive_worker(0, case, impl, 0, d)
-        else:
-            mp.spawn(_naive_worker, args=(case, impl, harness.free_port(), d), nprocs=case.world_size, join=True)
-        per_rank = [torch.load(os.path.join(d, f"rank{r}.pt")) for r in range(case.world_size)]
-    for r in range(1, case.world_size):
-        for a, b in zip(per_rank[0], per_rank[r]):
-            assert torch.equal(a, b), "final output must be identical on all ranks"
-    return per_rank[0]
-
-
-def _traj_worker(rank, case, port, outdir, num_steps, guidance):
-    harness._paths("oracle")
-    from oracle import workloads as W
-    from distrifuser_b200.compat.pipeline import SyntheticLatentPipeline
-    harness._init(rank, case.world_size, port)
-    cfg = naive_config(case, rank)
-    if case.world_size > 1:
-        harness._groups(cfg)
-    ucfg = W.unet_config(case.family)
-    model = OracleNaivePatchUNet(W.make_unet(case.family, case.weight_seed), cfg)
-    pipe = SyntheticLatentPipeline(harness._OracleUNetAdapter(model, model.config),
-                                   sdxl=ucfg.get("addition_embed_type") == "text_time", device="cpu", dtype=torch.float32)
-    model.set_counter(0)
-    g = torch.Generator().manual_seed(case.input_seed)
-    with torch.no_grad():
-        lat = pipe(prompt="a photo", height=8 * case.latent, width=8 * case.latent, num_inference_steps=num_steps,
-                   guidance_scale=guidance, generator=g).images
-    torch.save(lat, os.path.join(outdir, f"rank{rank}.pt"))
-    if case.world_size > 1:
-        dist.barrier()
-        dist.destroy_process_group()
-
-
-def run_naive_trajectory(case, num_steps=8, guidance=5.0):
-    """Final latents of a `num_steps` Euler trajectory with the naive-patch ORACLE UNet (fp32 CPU) -> [1,4,S,S]."""
-    with tempfile.TemporaryDirectory() as d:
-        if case.world_size == 1:
-            _traj_worker(0, case, 0, d, num_steps, guidance)
-        else:
-            mp.spawn(_traj_worker, args=(case, harness.free_port(), d, num_steps, guidance), nprocs=case.world_size,
-                     join=True)
-        outs = [torch.load(os.path.join(d, f"rank{r}.pt")) for r in range(case.world_size)]
-    for o in outs[1:]:
-        assert torch.equal(o, outs[0])
-    return outs[0]
-
-
-def main():
-    ap = argparse.ArgumentParser()
-    ap.add_argument("--case", default=None)
-    a = ap.parse_args()
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    golden = os.path.join(root, "tests", "golden")
-    os.makedirs(golden, exist_ok=True)
-    for case in NAIVE_CASES:
-        if a.case and case.name != a.case:
-            continue
-        t0 = time.time()
-        outs = run_naive_unet(case, impl="reference")
-        torch.save({"case": case.__dict__, "outs": [o.clone() for o in outs],
-                    "source": "reference NaivePatchUNet @ /root/reference over oracle/diffusers_stub, gloo, fp32"},
-                   os.path.join(golden, f"{case.name}.pt"))
-        print(f"{case.name}: {time.time() - t0:.1f}s  std={outs[-1].std():.4f}", flush=True)
-
-
-if __name__ == "__main__":
-    main()

@@ -10,6 +10,14 @@ behaviour, each piece citing the reference file:line it follows:
   * OracleCrossAttention  <- distrifuser/modules/pp/attn.py:42-104
   * OracleUNetPP          <- distrifuser/models/distri_sdxl_unet_pp.py:16-210 (eager path)
 
+Uneven row strips.  The reference asserts equal strips; these modules also restate the product's rule for a patch count
+that does not divide the latent rows (distrifuser_b200.utils.split_units, restated here so that the check stays
+independent): patch rank r of n holds `units[r]` units of 2^downsamplers latent rows, U // n each and one more for the
+first U % n ranks.  K/V slots then hold segments of unequal length, every GroupNorm mean over ranks weighs rank s by
+rows_s / sum(rows), and the conv_in slice and the final gather sit at the prefix sums of the rows.  Equal strips take the
+reference's expressions unchanged.  `bessel=False` drops the local-count Bessel factor, so that an uneven full_sync run
+equals the one-device UNet exactly.
+
 PINNING: this restatement is checked against outputs of the UNMODIFIED reference modules executed in the
 build container (oracle/make_golden.py imports them from /root/reference through oracle/diffusers_stub and
 runs them under gloo); the resulting vectors are committed in tests/golden/ and compared in
@@ -31,12 +39,23 @@ from torch.nn import functional as F
 
 
 # ----------------------------------------------------------------------------------------------- comm
+def _all_gather_padded(local: torch.Tensor, sizes: list[int], dim: int, group) -> list[torch.Tensor]:
+    """all_gather of tensors whose length along `dim` differs between the members (`sizes`): padded to the longest."""
+    shape = list(local.shape)
+    shape[dim] = max(sizes)
+    padded = local.new_zeros(shape)
+    padded.narrow(dim, 0, local.shape[dim]).copy_(local)
+    bufs = [torch.empty_like(padded) for _ in sizes]
+    dist.all_gather(bufs, padded, group=group)
+    return [b.narrow(dim, 0, sz).contiguous() for b, sz in zip(bufs, sizes)]
+
+
 class OracleComm:
     """Per-tensor peer slots with 1-step-stale visibility (utils.py:112-199)."""
 
     def __init__(self, cfg):
         self.cfg = cfg
-        self.shapes: list[tuple] = []
+        self.shapes: list[list[tuple]] = []                # per tensor, the shape of each source's slot
         self.slots: list[list[torch.Tensor]] | None = None
         self.pending: dict[int, torch.Tensor] = {}
 
@@ -44,16 +63,25 @@ class OracleComm:
     def n(self):
         return self.cfg.n_device_per_batch
 
-    def register(self, shape) -> int:                      # utils.py:130-149
-        self.shapes.append(tuple(shape))
+    def register(self, shape, lens=None) -> int:           # utils.py:130-149
+        """`lens`: each source's length along dim 1 (K/V of uneven strips); default: every source holds `shape`."""
+        shape = tuple(shape)
+        self.shapes.append([shape] * self.n if lens is None else [(shape[0], L, *shape[2:]) for L in lens])
         return len(self.shapes) - 1
 
     def create(self, dtype=torch.float32):                 # utils.py:151-164
-        self.slots = [[torch.zeros(s, dtype=dtype) for _ in range(self.n)] for s in self.shapes]
+        self.slots = [[torch.zeros(s, dtype=dtype) for s in shapes] for shapes in self.shapes]
+
+    def _all_gather(self, idx: int, local: torch.Tensor):
+        shapes = self.shapes[idx]
+        if len(set(shapes)) == 1:
+            dist.all_gather(self.slots[idx], local, group=self.cfg.batch_group)
+        else:
+            self.slots[idx] = _all_gather_padded(local, [s[1] for s in shapes], 1, self.cfg.batch_group)
 
     def gather_now(self, idx: int, local: torch.Tensor):
         """Blocking all_gather of a synchronous step (attn.py:133, conv2d.py:93, groupnorm.py:46)."""
-        dist.all_gather(self.slots[idx], local.contiguous(), group=self.cfg.batch_group)
+        self._all_gather(idx, local.contiguous())
         return self.slots[idx]
 
     def publish(self, idx: int, local: torch.Tensor):      # utils.py:181-190 (enqueue)
@@ -62,11 +90,14 @@ class OracleComm:
     def begin_step(self):
         """Make everything published during the previous step visible (utils.py:170-179,183-184)."""
         for idx in sorted(self.pending):
-            dist.all_gather(self.slots[idx], self.pending[idx], group=self.cfg.batch_group)
+            self._all_gather(idx, self.pending[idx])
         self.pending = {}
 
 
 class _Wrapped(nn.Module):                                 # modules/base_module.py:6-29
+    units: list[int] | None = None                         # row plan, set by OracleUNetPP (None: equal strips)
+    bessel: bool = True
+
     def __init__(self, module, cfg):
         super().__init__()
         self.module, self.cfg = module, cfg
@@ -85,6 +116,18 @@ class _Wrapped(nn.Module):                                 # modules/base_module
 
     def _bound(self):
         return self.comm is not None and self.comm.slots is not None and self.idx is not None
+
+    def rows(self, h):
+        """Rows of every patch rank where this rank holds h rows (tokens alike): distrifuser_b200.utils.patch_rows."""
+        units = self.units or [1] * self.cfg.n_device_per_batch
+        return [u * h // units[self.cfg.split_idx()] for u in units]
+
+    def row_weights(self, h):
+        """Each patch rank's share of the rows for uneven strips; None for equal strips (the reference's 1/n)."""
+        if self.units is None or len(set(self.units)) == 1:
+            return None
+        rows = self.rows(h)
+        return [s / sum(rows) for s in rows]
 
 
 # ----------------------------------------------------------------------------------------------- GroupNorm
@@ -106,33 +149,41 @@ class OracleGroupNorm(_Wrapped):
         x5 = x.reshape(b, G, c // G, h, w)
         mine = _moments(x5)                                                         # groupnorm.py:38-41 / 75-78
         n, r = cfg.n_device_per_batch, cfg.split_idx()
+        wts = self.row_weights(h)
+        avg = (lambda parts: sum(parts) / n) if wts is None else (lambda parts: sum(wt * g for wt, g in zip(wts, parts)))
         use_local_fallback = False
         if stat_modes:
             if not self._bound():
                 full = mine                                                         # groupnorm.py:43-44
             elif self._is_sync():
-                full = sum(self.comm.gather_now(self.idx, mine)) / n                # groupnorm.py:45-47
+                full = avg(self.comm.gather_now(self.idx, mine))                    # groupnorm.py:45-47
             else:
                 stale = self.comm.slots[self.idx]
                 if cfg.mode == "corrected_async_gn":                                # groupnorm.py:49-51
-                    full = sum(stale) / n + (mine - stale[r])
+                    full = avg(stale) + (mine - stale[r])
                     use_local_fallback = True
-                else:                                                               # groupnorm.py:52-55
+                elif wts is None:                                                   # groupnorm.py:52-55
                     full = (sum(stale) - stale[r] + mine) / n
+                else:
+                    full = avg([mine if s == r else g for s, g in enumerate(stale)])
                 self.comm.publish(self.idx, mine)                                   # groupnorm.py:56
             if cfg.mode == "corrected_async_gn":
                 use_local_fallback = True                                           # groupnorm.py:60-63 (all steps)
-        else:                                                                       # groupnorm.py:74-80
+        elif wts is None:                                                           # groupnorm.py:74-80
             full = mine.clone()
             if n > 1:
                 dist.all_reduce(full, op=dist.ReduceOp.SUM, group=cfg.batch_group)
             full = full / n
+        else:
+            full = mine * wts[r]
+            dist.all_reduce(full, op=dist.ReduceOp.SUM, group=cfg.batch_group)
         mean, meansq = full[0], full[1]
         var = meansq - mean * mean
         if use_local_fallback:
             var = torch.where(var < 0, mine[1] - mine[0] * mine[0], var)
         ne = (c // G) * h * w
-        var = var * (ne / (ne - 1))                                                 # groupnorm.py:65-66,84-85
+        if self.bessel:
+            var = var * (ne / (ne - 1))                                             # groupnorm.py:65-66,84-85
         y = ((x5 - mean) / (var + m.eps).sqrt()).reshape(b, c, h, w)                # groupnorm.py:67-69
         if m.affine:
             y = y * m.weight.view(1, -1, 1, 1) + m.bias.view(1, -1, 1, 1)           # groupnorm.py:70-72
@@ -150,9 +201,10 @@ class OracleConv2d(_Wrapped):
         m, cfg = self.module, self.cfg
         s, p = m.stride[0], m.padding[0]
         H = x.shape[2]
-        out_h = H // s // cfg.n_device_per_batch
         r = cfg.split_idx()
-        lo, hi = out_h * r * s - p, out_h * (r + 1) * s + p
+        units = self.units or [1] * cfg.n_device_per_batch
+        rows = self.rows(H // s * units[r] // sum(units))                           # output rows of every rank
+        lo, hi = sum(rows[:r]) * s - p, sum(rows[:r + 1]) * s + p
         pad_top, pad_bot = max(0, -lo), max(0, hi - H)
         xs = F.pad(x[:, :, max(lo, 0):min(hi, H)], [p, p, pad_top, pad_bot])
         return F.conv2d(xs, m.weight, m.bias, stride=s)
@@ -209,7 +261,7 @@ class OracleSelfAttention(_Wrapped):
         q = attn.to_q(hidden_states)                                                # attn.py:121
         kv = torch.cat([attn.to_k(hidden_states), attn.to_v(hidden_states)], -1)    # attn.py:23-39,125 (fused to_kv)
         if n > 1 and self.comm is not None and self.idx is None and self.comm.slots is None:
-            self.idx = self.comm.register((b, l, kv.shape[-1]))                     # attn.py:185-190
+            self.idx = self.comm.register((b, l, kv.shape[-1]), self.rows(l))       # attn.py:185-190
         if n == 1:
             full = kv                                                               # attn.py:127-128
         elif not self._bound():
@@ -269,14 +321,25 @@ def wrap_unet(model, cfg):
 
 
 class OracleUNetPP(nn.Module):
-    """Eager path of DistriUNetPP.forward (distri_sdxl_unet_pp.py:117-210) + BaseModel (base_model.py:8-52)."""
+    """Eager path of DistriUNetPP.forward (distri_sdxl_unet_pp.py:117-210) + BaseModel (base_model.py:8-52), with the row
+    plan of uneven strips (DistriUNetPP.row_plan)."""
 
-    def __init__(self, model, cfg):
+    def __init__(self, model, cfg, bessel=True):
         super().__init__()
         self.model = wrap_unet(model, cfg)
         self.cfg = cfg
         self.comm = None
         self.counter = 0
+        self.units = None
+        n = cfg.n_device_per_batch
+        if cfg.world_size > 1 and n > 1:
+            u = 2 ** sum(1 for blk in self.model.down_blocks if getattr(blk, "downsamplers", None) is not None)
+            S = cfg.height // 8
+            assert S % u == 0 and S // u >= n
+            U = S // u
+            self.units = [U // n + (1 if k < U % n else 0) for k in range(n)]
+        for m in self.wrapped():
+            m.units, m.bessel = self.units, bessel
 
     def wrapped(self):
         return [m for m in self.model.modules() if isinstance(m, _Wrapped)]
@@ -323,9 +386,13 @@ class OracleUNetPP(nn.Module):
                     added_cond_kwargs = {k: v[i:i + 1] for k, v in added_cond_kwargs.items()}
             out = self.model(sample, timestep, encoder_hidden_states, added_cond_kwargs=added_cond_kwargs,
                              return_dict=False)[0].contiguous()
-            parts = [torch.empty_like(out) for _ in range(cfg.world_size)]
-            dist.all_gather(parts, out)                                             # :166,191 (world group)
             n = cfg.n_device_per_batch
+            if self.units is None or len(set(self.units)) == 1:
+                parts = [torch.empty_like(out) for _ in range(cfg.world_size)]
+                dist.all_gather(parts, out)                                         # :166,191 (world group)
+            else:                                                                   # strips of unequal height
+                heights = [h * self.units[q % n] // sum(self.units) for q in range(cfg.world_size)]
+                parts = _all_gather_padded(out, heights, 2, None)
             if split:                                                               # :167-168
                 out = torch.cat([torch.cat(parts[:n], 2), torch.cat(parts[n:], 2)], 0)
             else:                                                                   # :192

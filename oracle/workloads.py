@@ -2,8 +2,9 @@
 (oracle/make_golden.py, runs the REAL reference), the oracle restatement (oracle/pp_modules.py) and the
 GPU parity tests.  Everything is regenerated from integer seeds so fixtures only store outputs.
 
-Inputs follow SURVEY.md 8(d): sample = randn([B,4,S,S]); encoder_hidden_states = randn([B,77,cross]);
-text_embeds = randn([B,pooled]); time_ids = [H,W,0,0,H,W]  (reference: pipelines.py:73-75,106-112).
+Inputs follow SURVEY.md 8(d): sample = randn([B,4,S,T]) (S = T but for the uneven-strip cases);
+encoder_hidden_states = randn([B,77,cross]); text_embeds = randn([B,pooled]); time_ids = [H,W,0,0,H,W]
+(reference: pipelines.py:73-75,106-112).
 """
 from __future__ import annotations
 
@@ -21,15 +22,15 @@ class DuckConfig:
     Field and method semantics restated from utils.py:52-110."""
 
     def __init__(self, world_size, rank, *, height, width, do_classifier_free_guidance=True, split_batch=True,
-                 warmup_steps=4, comm_checkpoint=60, mode="corrected_async_gn", batch_group=None,
-                 device="cpu"):
+                 warmup_steps=4, comm_checkpoint=60, mode="corrected_async_gn", parallelism="patch", split_scheme="row",
+                 batch_group=None, device="cpu"):
         self.world_size, self.rank = world_size, rank
         self.height, self.width = height, width
         self.do_classifier_free_guidance = do_classifier_free_guidance
         self.split_batch = split_batch
         self.warmup_steps, self.comm_checkpoint, self.mode = warmup_steps, comm_checkpoint, mode
         self.use_cuda_graph = False
-        self.parallelism, self.split_scheme, self.verbose = "patch", "row", False
+        self.parallelism, self.split_scheme, self.verbose = parallelism, split_scheme, False
         if do_classifier_free_guidance and split_batch:          # utils.py:68-75
             n = world_size // 2
             if n == 0:
@@ -52,8 +53,23 @@ class DuckConfig:
         return rank % self.n_device_per_batch
 
 
+class _PatchCase:
+    """What the drivers read from a patch-parallel case beyond its fields.  Methods and properties, not fields: the golden
+    fixtures pin each case type's fields (`gold["case"] == case.__dict__`)."""
+
+    @property
+    def batch(self):
+        return 2 if self.cfg else 1
+
+    def config_kwargs(self) -> dict:
+        """Keywords of DistriConfig (and of the oracle's DuckConfig) for this case."""
+        H, W = self.hw
+        return dict(height=8 * H, width=8 * W, do_classifier_free_guidance=self.cfg, split_batch=self.split_batch,
+                    warmup_steps=self.warmup_steps, comm_checkpoint=self.comm_checkpoint, mode=self.mode)
+
+
 @dataclasses.dataclass(frozen=True)
-class UNetCase:
+class UNetCase(_PatchCase):
     """One end-to-end tiny-UNet parity case."""
     name: str
     family: str = "tiny_sdxl"        # tiny_sdxl | tiny_sd15
@@ -69,8 +85,9 @@ class UNetCase:
     input_seed: int = 1234
 
     @property
-    def batch(self):
-        return 2 if self.cfg else 1
+    def hw(self):
+        """Latent rows and columns (image side / 8)."""
+        return self.latent, self.latent
 
 
 UNET_CASES = (
@@ -90,6 +107,29 @@ UNET_CASES = (
 )
 
 
+@dataclasses.dataclass(frozen=True)
+class RaggedCase(_PatchCase):
+    """A patch-parallel case at a latent of lat_h x lat_w, where the patch count need not divide the latent height into
+    equal strips (the reference asserts equal strips, so these cases have no reference goldens)."""
+    name: str
+    family: str = "tiny_sdxl"
+    world_size: int = 2
+    cfg: bool = True
+    split_batch: bool = False
+    mode: str = "corrected_async_gn"
+    warmup_steps: int = 1
+    steps: int = 4
+    lat_h: int = 36                  # latent rows (image height / 8)
+    lat_w: int = 28
+    comm_checkpoint: int = 20
+    weight_seed: int = 0
+    input_seed: int = 4321
+
+    @property
+    def hw(self):
+        return self.lat_h, self.lat_w
+
+
 def unet_config(family: str) -> dict:
     from diffusers.models.unet_2d_condition import (sd15_config, sdxl_config, tiny_sd15_config,
                                                     tiny_sdxl_config)
@@ -105,11 +145,11 @@ def make_unet(family: str, seed: int = 0, dtype=torch.float32):
     return unet.to(dtype).eval()
 
 
-def unet_inputs(case: UNetCase, step: int, cfg_dict: dict, dtype=torch.float32):
-    """Inputs of denoise call `step` (full CFG batch, as the diffusers loop hands them to the UNet)."""
+def unet_inputs(case, step: int, cfg_dict: dict, dtype=torch.float32):
+    """Inputs of denoise call `step` (full CFG batch, as the diffusers loop hands them to the UNet) at the case's latent."""
     g = torch.Generator().manual_seed(case.input_seed + 7919 * step)
-    B, S = case.batch, case.latent
-    sample = torch.randn(B, 4, S, S, generator=g)
+    B, (S, T) = case.batch, case.hw
+    sample = torch.randn(B, 4, S, T, generator=g)
     g2 = torch.Generator().manual_seed(case.input_seed)            # prompt embeddings are constant per image
     ehs = torch.randn(B, 77, cfg_dict["cross_attention_dim"], generator=g2)
     timestep = torch.full((B,), 981 - 20 * step, dtype=torch.long)
@@ -117,8 +157,8 @@ def unet_inputs(case: UNetCase, step: int, cfg_dict: dict, dtype=torch.float32):
     if cfg_dict.get("addition_embed_type") == "text_time":
         pooled = cfg_dict["projection_class_embeddings_input_dim"] - 6 * cfg_dict["addition_time_embed_dim"]
         text = torch.randn(B, pooled, generator=g2)
-        H = float(8 * S)
-        ids = torch.tensor([[H, H, 0.0, 0.0, H, H]] * B)
+        H, W = float(8 * S), float(8 * T)
+        ids = torch.tensor([[H, W, 0.0, 0.0, H, W]] * B)
         added = {"text_embeds": text.to(dtype), "time_ids": ids.to(dtype)}
     return dict(sample=sample.to(dtype), timestep=timestep, encoder_hidden_states=ehs.to(dtype),
                 added_cond_kwargs=added)

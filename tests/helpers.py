@@ -146,3 +146,27 @@ def _close(out, ref, rel=2e-3, abs_=4e-3):
     err = (out.float() - ref).abs()
     bad = err > (abs_ + rel * ref.abs())
     assert not bad.any(), f"max err {err.max().item():.4e} at ref {ref.flatten()[err.flatten().argmax()].item():.3f}; {int(bad.sum())} bad"
+
+
+def psnr(a, ref, floor=1e-20):
+    """PSNR of `a` against `ref` in dB, peak = max |ref| (the reference's metric, scripts/compute_metrics.py:62-79)."""
+    mse = ((a - ref) ** 2).mean().item()
+    return 10 * torch.log10(ref.abs().max() ** 2 / max(mse, floor)).item()
+
+
+def check_parity(name, outs, want, ranks_identical=False):
+    """Product eps predictions (per rank, per step) against golden or oracle ones (per step): fp16 with fp32 accumulation
+    against fp32, on outputs of std ~0.35: mean |err| < 4e-3, max |err| < 4e-2 and PSNR > 45 dB every step.
+    `ranks_identical`: every rank also holds rank 0's output bit for bit."""
+    for r, per_rank in enumerate(outs):
+        assert len(per_rank) == len(want), f"{name} rank{r}: {len(per_rank)} steps, want {len(want)}"
+        for t, (a, b) in enumerate(zip(per_rank, want)):
+            assert a.shape == b.shape
+            err = (a - b).abs()
+            p = psnr(a, b)
+            assert err.mean().item() < 4e-3 and err.max().item() < 4e-2 and p > 45, \
+                f"{name} rank{r} step{t}: mean {err.mean():.2e} max {err.max():.2e} psnr {p:.1f} dB"
+    if ranks_identical:
+        for r, per_rank in enumerate(outs[1:], 1):
+            for t, (a, b) in enumerate(zip(per_rank, outs[0])):
+                assert torch.equal(a, b), f"{name}: rank {r} differs from rank 0 at step {t}"

@@ -9,13 +9,9 @@ import torch
 from torch import distributed as dist
 from torch import multiprocessing as mp
 
+from helpers import psnr
 from oracle import harness, workloads
 from oracle.naive_patch import NAIVE_CASES, NaiveCase, run_naive_trajectory, run_naive_unet
-
-
-def _psnr(a, ref):
-    mse = ((a - ref) ** 2).mean().item()
-    return 10 * torch.log10(ref.abs().max() ** 2 / max(mse, 1e-30)).item()
 
 
 @pytest.mark.parametrize("case", NAIVE_CASES, ids=lambda c: c.name)
@@ -80,10 +76,10 @@ def test_naive_patch_premise_on_trajectories():
     1-step-stale method on data it never saw."""
     steps = 8
     full = run_naive_trajectory(NaiveCase("one_device", world_size=1), num_steps=steps)
-    naive = {s: _psnr(run_naive_trajectory(NaiveCase(f"n2_{s}", world_size=2, scheme=s), num_steps=steps), full)
+    naive = {s: psnr(run_naive_trajectory(NaiveCase(f"n2_{s}", world_size=2, scheme=s), num_steps=steps), full, floor=1e-30)
              for s in ("row", "col", "alternate")}
-    distri = _psnr(harness.run_trajectory(workloads.UNetCase("pp_n2", world_size=2, split_batch=False, warmup_steps=1),
-                                          num_steps=steps), full)
+    distri = psnr(harness.run_trajectory(workloads.UNetCase("pp_n2", world_size=2, split_batch=False, warmup_steps=1),
+                                         num_steps=steps), full, floor=1e-30)
     print(f"PSNR vs one device: naive n=2 {naive}, DistriFusion n=2 {distri:.1f} dB")
     assert all(p < 40 for p in naive.values()), naive
     assert distri > 50, distri

@@ -3,63 +3,47 @@ output gather) against the golden vectors of the unmodified reference NaivePatch
 API against the naive-patch oracle trajectory, and df_output_gather_2d against a torch placement, bit for bit.
 
 Multi-rank cases run on real GPUs when the box has them; otherwise the ranks share cuda:0 through CUDA IPC.  Tolerances are
-those of test_unet_gpu.py: mean |err| < 4e-3, max |err| < 4e-2 and PSNR > 45 dB per step."""
+those of test_unet_gpu.py (helpers.check_parity): mean |err| < 4e-3, max |err| < 4e-2 and PSNR > 45 dB per step."""
 import os
 
 import pytest
 import torch
 
-from helpers import LoopbackArena
-from mp_naive import run_naive_product_trajectory, run_naive_product_unet
+from helpers import LoopbackArena, check_parity, psnr
+from mp_product import run_product_trajectory, run_product_unet
 from oracle.naive_patch import NAIVE_CASES, NaiveCase, run_naive_trajectory
 
 pytestmark = pytest.mark.gpu
 CASES = {c.name: c for c in NAIVE_CASES}
 
 
-def _psnr(a, ref):
-    mse = ((a - ref) ** 2).mean().item()
-    return 10 * torch.log10(ref.abs().max() ** 2 / max(mse, 1e-20)).item()
-
-
 def _check(name, outs, gold_path):
-    gold = torch.load(gold_path)["outs"]
-    for r, per_rank in enumerate(outs):
-        assert len(per_rank) == len(gold)
-        for t, (a, b) in enumerate(zip(per_rank, gold)):
-            assert a.shape == b.shape
-            err = (a - b).abs()
-            psnr = _psnr(a, b)
-            assert err.mean().item() < 4e-3 and err.max().item() < 4e-2 and psnr > 45, \
-                f"{name} rank{r} step{t}: mean {err.mean():.2e} max {err.max():.2e} psnr {psnr:.1f} dB"
-    for per_rank in outs[1:]:
-        for a, b in zip(per_rank, outs[0]):
-            assert torch.equal(a, b), f"{name}: ranks disagree on the gathered output"
+    check_parity(name, outs, torch.load(gold_path)["outs"], ranks_identical=True)
 
 
 @pytest.mark.parametrize("name", ["naive_sdxl_w2_row", "naive_sdxl_w4_col_split", "naive_sdxl_w2_alternate",
                                   "naive_sdxl_w4_alternate", "naive_sd15_w4_col"])
 def test_naive_unet_vs_reference(name, golden_dir):
-    _check(name, run_naive_product_unet(CASES[name]), os.path.join(golden_dir, f"{name}.pt"))
+    _check(name, run_product_unet(CASES[name]), os.path.join(golden_dir, f"{name}.pt"))
 
 
 @pytest.mark.parametrize("name", ["naive_sdxl_w2_alternate", "naive_sdxl_w4_alternate"])
 def test_naive_unet_cuda_graph_vs_reference(name, golden_dir):
     """`alternate` with CUDA graphs: steps 0 and 2 replay the row-strip graph, steps 1 and 3 the column-strip graph."""
-    _check(name, run_naive_product_unet(CASES[name], use_graph=True), os.path.join(golden_dir, f"{name}.pt"))
+    _check(name, run_product_unet(CASES[name], use_graph=True), os.path.join(golden_dir, f"{name}.pt"))
 
 
 @pytest.mark.multigpu(8)
 def test_naive_unet_eight_gpus(golden_dir):
     name = "naive_sdxl_w8_split_col"
-    _check(name, run_naive_product_unet(CASES[name]), os.path.join(golden_dir, f"{name}.pt"))
+    _check(name, run_product_unet(CASES[name]), os.path.join(golden_dir, f"{name}.pt"))
 
 
 @pytest.mark.parametrize("use_graph", [False, True])
 def test_naive_world1_is_the_plain_unet(use_graph, golden_dir):
     """At world size 1 naive patch is the wrapped UNet on the whole image: the reference's one-GPU golden applies."""
     case = NaiveCase("w1", world_size=1, scheme="alternate")
-    _check("naive w1", run_naive_product_unet(case, use_graph=use_graph), os.path.join(golden_dir, "unet_sdxl_w1.pt"))
+    _check("naive w1", run_product_unet(case, use_graph=use_graph), os.path.join(golden_dir, "unet_sdxl_w1.pt"))
 
 
 @pytest.mark.parametrize("case", [NaiveCase("traj_sdxl_w2_alternate", world_size=2, scheme="alternate"),
@@ -69,14 +53,14 @@ def test_naive_pipeline_trajectory(case):
     """DistriSDXLPipeline / DistriSDPipeline.from_synthetic(DistriConfig(parallelism="naive_patch", ...)) with CUDA graphs,
     8 Euler steps: the final latents are bit-identical on every rank and between two images of one seed (asserted in the
     worker), and within 35 dB of the fp32 naive-patch oracle trajectory."""
-    got = run_naive_product_trajectory(case, num_steps=8)
+    got = run_product_trajectory(case, num_steps=8)
     for lat in got[1:]:
         assert torch.equal(lat, got[0]), "ranks hold different latents"
     want = run_naive_trajectory(case, num_steps=8)
     assert got[0].shape == want.shape
-    psnr = _psnr(got[0], want)
-    print(f"{case.name}: product vs oracle trajectory {psnr:.1f} dB")
-    assert torch.isfinite(got[0]).all() and psnr > 35, f"{psnr:.1f} dB"
+    p = psnr(got[0], want)
+    print(f"{case.name}: product vs oracle trajectory {p:.1f} dB")
+    assert torch.isfinite(got[0]).all() and p > 35, f"{p:.1f} dB"
 
 
 # ================================================================================================================ output gather

@@ -8,15 +8,11 @@ import dataclasses
 import pytest
 import torch
 
+from helpers import psnr
 from oracle import harness, workloads
 from mp_product import run_product_trajectory
 
 pytestmark = pytest.mark.gpu
-
-
-def _psnr(a, b):
-    mse = ((a - b) ** 2).mean().item()
-    return 10 * torch.log10(b.abs().max() ** 2 / max(mse, 1e-20)).item()
 
 
 @pytest.mark.parametrize("name,graph", [("sdxl_w1", True), ("sdxl_w2_nosplit", True),
@@ -29,7 +25,7 @@ def test_trajectory_matches_oracle(name, graph):
         assert lat.shape == want.shape == (1, 4, case.latent, case.latent)
         assert torch.isfinite(lat).all()
         assert torch.equal(lat, got[0]), "every rank must hold the same latents"
-        p = _psnr(lat, want)
+        p = psnr(lat, want)
         assert p > 35.0, f"{name} rank{r}: PSNR {p:.1f} dB vs the fp32 oracle trajectory"
 
 

@@ -9,8 +9,8 @@ import torch
 from torch import distributed as dist
 from torch import multiprocessing as mp
 
-from mp_ragged import RaggedCase, run_oracle_unet
-from oracle.harness import free_port
+from oracle.harness import free_port, run_unet
+from oracle.workloads import RaggedCase
 
 
 def test_split_units_rule():
@@ -106,9 +106,8 @@ EXACT = [
 def test_uneven_full_sync_equals_one_device(case, units):
     """Without the local-count Bessel factor, full_sync over uneven strips is the whole-image UNet (fp32, within 1e-5)."""
     import dataclasses
-    got, plan = run_oracle_unet(case, bessel=False)
-    assert plan == units
-    want, _ = run_oracle_unet(dataclasses.replace(case, world_size=1), bessel=False)
+    got = run_unet(case, bessel=False, row_units=units)
+    want = run_unet(dataclasses.replace(case, world_size=1), bessel=False)
     for t, (a, b) in enumerate(zip(got, want)):
         assert a.shape == b.shape == (2, 4, case.lat_h, case.lat_w)
         err = (a - b).abs().max().item()
@@ -118,9 +117,8 @@ def test_uneven_full_sync_equals_one_device(case, units):
 @pytest.mark.parametrize("world,units", [(2, [5, 4]), (4, [3, 2, 2, 2])])
 def test_uneven_corrected_warmup_equals_full_sync(world, units):
     """With the Bessel factor, the synchronous warm-up steps of corrected_async_gn compute what full_sync computes."""
-    sync, plan = run_oracle_unet(RaggedCase("full", world_size=world, mode="full_sync", warmup_steps=2, steps=3))
-    corr, _ = run_oracle_unet(RaggedCase("corr", world_size=world, mode="corrected_async_gn", warmup_steps=2, steps=3))
-    assert plan == units
+    sync = run_unet(RaggedCase("full", world_size=world, mode="full_sync", warmup_steps=2, steps=3), row_units=units)
+    corr = run_unet(RaggedCase("corr", world_size=world, mode="corrected_async_gn", warmup_steps=2, steps=3), row_units=units)
     for t, (a, b) in enumerate(zip(corr, sync)):
         err = (a - b).abs().max().item()
         assert err < 1e-5, f"warm-up step {t}: max |err| {err:.2e}"

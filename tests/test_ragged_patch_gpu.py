@@ -3,15 +3,17 @@
 Kernels: the attention kernel over K/V segments of unequal length (df_attn_fwd_ragged) and the GroupNorm statistics combine
 with per-source weights (df_groupnorm_fwd_weighted / df_groupnorm_halo_fwd_weighted), each against an fp32 torch restatement
 at the tolerances of test_kernel_configs_gpu.py; with equal lengths / weights the new entry points must give the bits of the
-existing ones.  UNet and pipeline: the product against the uneven CPU oracle (tests/ragged_oracle.py), with test_unet_gpu.py's
-bars per step and test_pipeline_gpu.py's for a trajectory."""
+existing ones.  UNet and pipeline: the product against the CPU oracle on uneven strips (oracle/pp_modules.py), with
+test_unet_gpu.py's bars per step and test_pipeline_gpu.py's for a trajectory."""
 import ctypes as C
 
 import pytest
 import torch
 
-from helpers import LoopbackArena, _gn_ref, _moments, sdpa_ref
-from mp_ragged import RaggedCase, run_oracle_trajectory, run_oracle_unet, run_product_trajectory, run_product_unet
+from helpers import LoopbackArena, _gn_ref, _moments, check_parity, psnr, sdpa_ref
+from mp_product import run_product_trajectory, run_product_unet
+from oracle import harness
+from oracle.workloads import RaggedCase
 
 pytestmark = pytest.mark.gpu
 
@@ -335,20 +337,6 @@ def test_groupnorm_weighted_equal_weights_bit_identical(arenas, mode, halo):
 
 
 # ================================================================================================================ UNet, pipeline
-def _check_unet(name, product, oracle):
-    ranks = [outs for outs, _ in product]
-    for r in range(1, len(ranks)):
-        for t, (a, b) in enumerate(zip(ranks[0], ranks[r])):
-            assert torch.equal(a, b), f"{name}: rank {r} differs from rank 0 at step {t}"
-    for t, (a, b) in enumerate(zip(ranks[0], oracle)):
-        assert a.shape == b.shape
-        err = (a - b).abs()
-        mse = (err ** 2).mean().item()
-        psnr = 10 * torch.log10(b.abs().max() ** 2 / max(mse, 1e-20)).item()
-        assert err.mean().item() < 4e-3 and err.max().item() < 4e-2 and psnr > 45, \
-            f"{name} step{t}: mean {err.mean():.2e} max {err.max():.2e} psnr {psnr:.1f} dB"
-
-
 MODES = ("corrected_async_gn", "stale_gn", "sync_gn", "separate_gn", "full_sync", "no_sync")
 UNET = [pytest.param(RaggedCase(f"sdxl_n2_{m}", world_size=2, mode=m, steps=3), [5, 4], False, id=f"n2-{m}") for m in MODES] + [
     pytest.param(RaggedCase("sdxl_n4", world_size=4, steps=3), [3, 2, 2, 2], False, id="n4-nosplit"),
@@ -361,20 +349,16 @@ UNET = [pytest.param(RaggedCase(f"sdxl_n2_{m}", world_size=2, mode=m, steps=3), 
 @pytest.mark.parametrize("case,units,graph", UNET)
 def test_unet_uneven_strips(case, units, graph):
     """The product UNet over uneven strips against the uneven oracle, every step; all ranks agree bit for bit."""
-    product = run_product_unet(case, use_graph=graph)
-    assert all(u == units for _, u in product), f"row plan {[u for _, u in product]}"
-    oracle, plan = run_oracle_unet(case)
-    assert plan == units
-    _check_unet(case.name, product, oracle)
+    product = run_product_unet(case, use_graph=graph, row_units=units)
+    check_parity(case.name, product, harness.run_unet(case, row_units=units), ranks_identical=True)
 
 
 @pytest.mark.multigpu(8)
 def test_unet_uneven_strips_eight_gpus():
     """cfg2 x patch4 over [3, 2, 2, 2] units on 8 real GPUs."""
     case = RaggedCase("sdxl_w8_split", world_size=8, split_batch=True, steps=3)
-    product = run_product_unet(case)
-    assert all(u == [3, 2, 2, 2] for _, u in product)
-    _check_unet(case.name, product, run_oracle_unet(case)[0])
+    product = run_product_unet(case, row_units=[3, 2, 2, 2])
+    check_parity(case.name, product, harness.run_unet(case, row_units=[3, 2, 2, 2]), ranks_identical=True)
 
 
 def test_pipeline_uneven_height_trajectory():
@@ -384,8 +368,7 @@ def test_pipeline_uneven_height_trajectory():
     got = run_product_trajectory(case, num_steps=8)
     for g in got[1:]:
         assert torch.equal(g, got[0]), "ranks disagree on the final latents"
-    want = run_oracle_trajectory(case, num_steps=8)
+    want = harness.run_trajectory(case, num_steps=8)
     assert got[0].shape == want.shape == (1, 4, 36, 28)
-    mse = ((got[0] - want) ** 2).mean().item()
-    psnr = 10 * torch.log10(want.abs().max() ** 2 / max(mse, 1e-20)).item()
-    assert psnr > 35, f"trajectory PSNR {psnr:.1f} dB"
+    p = psnr(got[0], want)
+    assert p > 35, f"trajectory PSNR {p:.1f} dB"

@@ -9,6 +9,7 @@ import os
 import pytest
 import torch
 
+from helpers import check_parity, psnr
 from oracle import workloads
 from mp_product import run_product_unet
 
@@ -17,15 +18,7 @@ CASES = {c.name: c for c in workloads.UNET_CASES}
 
 
 def _check(case, outs, golden_dir):
-    gold = torch.load(os.path.join(golden_dir, f"unet_{case.name}.pt"))["outs"]
-    for r, per_rank in enumerate(outs):
-        for t, (a, b) in enumerate(zip(per_rank, gold)):
-            assert a.shape == b.shape                                          # identical latent shapes
-            err = (a - b).abs()
-            mse = (err ** 2).mean().item()
-            psnr = 10 * torch.log10(b.abs().max() ** 2 / max(mse, 1e-20)).item()
-            assert err.mean().item() < 4e-3 and err.max().item() < 4e-2 and psnr > 45, \
-                f"{case.name} rank{r} step{t}: mean {err.mean():.2e} max {err.max():.2e} psnr {psnr:.1f} dB"
+    check_parity(case.name, outs, torch.load(os.path.join(golden_dir, f"unet_{case.name}.pt"))["outs"])
 
 
 def test_unet_single_gpu(golden_dir):
@@ -84,11 +77,10 @@ def test_full_size_sdxl_unet_step_vs_oracle():
     assert got.shape == want.shape == (2, 4, 64, 64)
     err = (got - want).abs()
     std = want.std().item()
-    mse = (err ** 2).mean().item()
-    psnr = 10 * torch.log10(want.abs().max() ** 2 / max(mse, 1e-20)).item()
+    p = psnr(got, want)
     assert torch.isfinite(got).all()
-    assert err.mean().item() < 1.2e-2 * std and err.max().item() < 0.12 * std and psnr > 45, \
-        f"mean {err.mean():.2e} max {err.max():.2e} std {std:.3f} psnr {psnr:.1f} dB"
+    assert err.mean().item() < 1.2e-2 * std and err.max().item() < 0.12 * std and p > 45, \
+        f"mean {err.mean():.2e} max {err.max():.2e} std {std:.3f} psnr {p:.1f} dB"
 
 
 def test_unet_multi_rank_cuda_graph(golden_dir):
