@@ -32,7 +32,7 @@ def build(force: bool = False, verbose: bool = False, out: str | None = None, cs
     nvcc = shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
     if not os.path.exists(nvcc):
         raise RuntimeError("nvcc not found: cannot build libdistrifuser_b200.so")
-    extra = os.environ.get("DF_NVCC_FLAGS", "").split()          # e.g. -DDF_EMU_PAIRS_OF_8=0 for kernel experiments
+    extra = os.environ.get("DF_NVCC_FLAGS", "").split()          # e.g. -DDF_MBAR_DEBUG for kernel experiments
     cmd = [nvcc, *FLAGS, *extra, "-I", os.path.join(HERE, "..", "include"), "-o", out or LIB, *[os.path.join(csrc or CSRC, s) for s in SOURCES]]
     if verbose:
         cmd.insert(1, "-Xptxas=-v")

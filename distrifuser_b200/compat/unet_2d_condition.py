@@ -194,8 +194,7 @@ class ResnetBlock2D(nn.Module):
         self.temb_has_conv1_bias = False # ... which then already contains conv1.bias (conv1 runs without its bias pass)
 
     def folds_conv1_bias(self) -> bool:
-        from .. import ops
-        return self.fused_norm_act and ops.fused_conv_bias() and _conv_of(self.conv1).bias is not None
+        return self.fused_norm_act and _conv_of(self.conv1).bias is not None
 
     def _tail_bias(self):
         """conv2.bias + conv_shortcut.bias as one vector (cached on the parameters' versions): added together with the
@@ -227,10 +226,9 @@ class ResnetBlock2D(nn.Module):
         t = self.temb_proj if self.temb_proj is not None else self.time_emb_proj(self.nonlinearity(temb))
         if fused_tail:
             # shortcut without its bias pass; conv2 without bias; then conv2.bias + shortcut.bias + residual in one pass
-            from .. import ops
             sc = self.conv_shortcut
-            res = x if sc is None else F.conv2d(x, sc.weight, None if ops.fused_conv_bias() else sc.bias)
-            tail_bias = self._tail_bias() if ops.fused_conv_bias() else None
+            res = x if sc is None else F.conv2d(x, sc.weight)
+            tail_bias = self._tail_bias()
             if fused_halo and self.conv2.halo_plan(h) is not None:
                 return self.conv2.forward_padded(self.norm2(h, addend=t, pad_for=self.conv2), residual=res, bias=tail_bias)
             return self.conv2(self.norm2(h, addend=t), residual=res, bias=tail_bias)

@@ -86,9 +86,8 @@ struct SegInfo {
   int32_t tile0[DF_MAX_WORLD + 1]; // first tile of walk order o in the concatenated tile range; tile0[nseg] = all tiles
 };
 
-#ifndef DF_EMU_GROUPS
-#define DF_EMU_GROUPS 3      // of the 16 column groups of a tile row, this many (evenly spread) take the polynomial exp2 (FMA/ALU
-#endif                       // pipes) instead of MUFU
+// of the 16 column groups of a tile row, this many (evenly spread) take the polynomial exp2 (FMA/ALU pipes) instead of MUFU
+constexpr int kEmuGroups = 3;
 
 template <int N>
 __device__ __forceinline__ void wgmma_ss(float* d, uint64_t a_desc, uint64_t b_desc, uint32_t accumulate) {
@@ -167,7 +166,6 @@ fmha_fwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
-  pdl_wait();                                          // everything above overlapped the tail of the previous kernel
 
   if (warp >= WARP_TMA) {
     // =============================================================== scheduler + TMA producer
@@ -369,7 +367,7 @@ fmha_fwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
 #pragma unroll
             for (int k = 0; k < 4; ++k) {
               const float x = fmaf(s[4 * i + k], scale_log2, k < 2 ? nA : nB);
-              s[4 * i + k] = ((grp * DF_EMU_GROUPS) / 16 != ((grp + 1) * DF_EMU_GROUPS) / 16) ? ex2_poly(x) : ex2(x);
+              s[4 * i + k] = ((grp * kEmuGroups) / 16 != ((grp + 1) * kEmuGroups) / 16) ? ex2_poly(x) : ex2(x);
             }
             lA += s[4 * i] + s[4 * i + 1];
             lB += s[4 * i + 2] + s[4 * i + 3];
@@ -545,9 +543,7 @@ extern "C" int df_attn_make_kvmaps(df_comm_t comm, uint64_t tensor_off, uint64_t
 }
 
 namespace {
-#ifndef DF_MIN_PART_TILES
-#define DF_MIN_PART_TILES 8    // a part of a split unit keeps at least this many K/V tiles (Q load + partial write + merge per part)
-#endif
+constexpr int kMinPartTiles = 8;    // a part of a split unit keeps at least this many K/V tiles (Q load + partial write + merge per part)
 // Grid and work schedule of a launch (see the kernel): G resident CTAs, `a` whole units per CTA, R left-over units in P parts.
 // Policy: the left-over units of a grid that already fills the SMs are not cut -- the R CTAs of the last round have the memory
 // system to themselves, which a balanced tail would trade for partial writes and a merge -- so P > 1 only when the units leave
@@ -564,7 +560,7 @@ void plan_schedule(int b, int lq, int t_all, int heads, bool have_ws, int& grid,
     sc.dyn = have_ws ? 1 : 0;                          // the ticket counter lives in the workspace
   } else {
     long long p = have_ws ? slots / units : 1;
-    if (p > t_all / DF_MIN_PART_TILES) p = t_all / DF_MIN_PART_TILES;
+    if (p > t_all / kMinPartTiles) p = t_all / kMinPartTiles;
     if (p < 1) p = 1;
     sc.a = 0; sc.R = (int)units; sc.P = (int)p; sc.dyn = 0;
     grid = (int)(units * p);
@@ -639,9 +635,9 @@ int attn_fwd_impl(df_comm_t comm, const void* q, const void* kv_own, void* out, 
       DF_CHECK_CUDA(cudaFuncSetAttribute(fmha_fwd_kernel<NB>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes)); \
       attr_set = true;                                                                                                       \
     }                                                                                                                        \
-    DF_CHECK_CUDA(launch_pdl(PDL_ATTN, fmha_fwd_kernel<NB>, grid, dim3(NTHREADS), smem_bytes, (cudaStream_t)stream, tq, tkv,           \
-                             (const CUtensorMap*)kvmaps, comm, segs, (__half*)out, lq, heads, d, o_pitch, nseg,              \
-                             own_seg, idx, wait_flags, sc, sched, part_o, part_ml, part_cnt, sched_ctr));                               \
+    fmha_fwd_kernel<NB><<<grid, NTHREADS, smem_bytes, (cudaStream_t)stream>>>(                                             \
+        tq, tkv, (const CUtensorMap*)kvmaps, comm, segs, (__half*)out, lq, heads, d, o_pitch, nseg, own_seg, idx, wait_flags,  \
+        sc, sched, part_o, part_ml, part_cnt, sched_ctr);                                                                    \
   }
   if (nblk == 1) DF_LAUNCH_FMHA(1) else if (nblk == 2) DF_LAUNCH_FMHA(2) else DF_LAUNCH_FMHA(3)
 #undef DF_LAUNCH_FMHA

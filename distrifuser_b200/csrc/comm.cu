@@ -2,7 +2,6 @@
 // final epsilon gather.  Replaces PatchParallelismCommManager (distrifuser/utils.py:112-199) and the
 // blocking collectives of the pp modules (attn.py:133, conv2d.py:93, distri_sdxl_unet_pp.py:166,191).
 #include <stdarg.h>
-#include <stdlib.h>
 #include <string.h>
 
 #include "common.cuh"
@@ -16,16 +15,6 @@ void set_error(const char* fmt, ...) {
   va_end(ap);
 }
 }  // namespace df
-
-unsigned df::pdl_mask() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("DF_PDL");          // opt-in (off by default)
-    v = e ? atoi(e) : 0;
-    if (v < 0) v = 0;
-  }
-  return (unsigned)v;
-}
 
 using namespace df;
 
@@ -112,12 +101,10 @@ extern "C" int df_step_begin(uint32_t* clock, int kind, void* stream) {
 
 // ------------------------------------------------------------------------------------ publication
 // One load, `npeer` stores per 16-byte vector; the last CTA to finish stamps the peers' flags.
-// 128 threads, DF_PUB_UNROLL 16-byte loads in flight per thread: the transfer is bound by how many loads are outstanding (local
+// 128 threads, kPubUnroll 16-byte loads in flight per thread: the transfer is bound by how many loads are outstanding (local
 // read latency ~1 us; the peer stores are posted).  What is exposed is the tail of the step's last publications, so a faster
 // transfer wins over taking fewer SM slots.
-#ifndef DF_PUB_UNROLL
-#define DF_PUB_UNROLL 8
-#endif
+constexpr int kPubUnroll = 8;
 __global__ void __launch_bounds__(128, 8) publish_kernel(df_comm_t c, const char* __restrict__ src, uint64_t rows,
                                                           uint64_t vec_per_row, uint64_t src_pitch, uint64_t tensor_off,
                                                           uint64_t slot_bytes, int idx, uint32_t peer_mask) {
@@ -125,7 +112,7 @@ __global__ void __launch_bounds__(128, 8) publish_kernel(df_comm_t c, const char
   const uint64_t total = rows * vec_per_row;
   const uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
   const uint64_t slot_off = slot_offset(c, epoch, tensor_off, slot_bytes, c.rank);
-  constexpr int U = DF_PUB_UNROLL;
+  constexpr int U = kPubUnroll;
   uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
   for (; i + (U - 1) * stride < total; i += U * stride) {
     int4 v[U];

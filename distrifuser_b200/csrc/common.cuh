@@ -64,15 +64,13 @@ __device__ __forceinline__ uint64_t globaltimer_ns() {
   asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t));
   return t;
 }
-#ifndef DF_SPIN_TIMEOUT_NS
-#define DF_SPIN_TIMEOUT_NS 30000000000ull  // a peer that never arrives becomes a CUDA error, not a hung GPU
-#endif
+constexpr uint64_t kSpinTimeoutNs = 30000000000ull;  // a peer that never arrives becomes a CUDA error, not a hung GPU
 // kReport = false drops the printf before the trap: a kernel that issues wgmma must contain no function call (printf is one),
 // or ptxas serialises every wgmma of the kernel (warning C7510).
 template <bool kReport = true>
 __device__ __forceinline__ void spin_until(const uint32_t* flag, uint32_t want, uint64_t timeout_ns = 0) {
   if (epoch_reached(ld_acquire_sys(flag), want)) return;
-  if (timeout_ns == 0) timeout_ns = DF_SPIN_TIMEOUT_NS;
+  if (timeout_ns == 0) timeout_ns = kSpinTimeoutNs;
   const uint64_t t0 = globaltimer_ns();
   uint32_t polls = 0;
   while (!epoch_reached(ld_acquire_sys(flag), want)) {
@@ -100,32 +98,6 @@ __device__ __forceinline__ int4 ld_v4(const void* p) {
 }
 __device__ __forceinline__ void st_v4(void* p, const int4& v) {
   asm volatile("st.global.v4.s32 [%0], {%1,%2,%3,%4};" ::"l"(p), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
-}
-
-// ------------------------------------------------------------------ programmatic dependent launch (PDL)
-// A denoise step is a chain of ~1 400 short kernels; with the launch attribute below a kernel of this library may be scheduled
-// while its predecessor in the stream is still draining, run its prologue (barrier set-up, tensor-map prefetch, index
-// arithmetic) and then block in pdl_wait() until the predecessor has completed and flushed its writes.  No global memory is
-// read or written before pdl_wait().  Opt-in per kernel family with the DF_PDL bit mask (without the attribute the device-side wait
-// is a no-op).
-unsigned pdl_mask();   // DF_PDL bit mask: 1 attention, 2 add+LayerNorm / GEGLU, 4 GroupNorm, 8 GEMM (0 = off, default)
-enum { PDL_ATTN = 1, PDL_ELEM = 2, PDL_GN = 4, PDL_GEMM = 8 };
-
-__device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
-
-template <typename... KArgs, typename... Args>
-inline cudaError_t launch_pdl(unsigned family, void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args... args) {
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = grid;
-  cfg.blockDim = block;
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = st;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = (pdl_mask() & family) ? 1 : 0;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  return cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
 }
 
 // ------------------------------------------------------------------ cross-rank protocol (include/distrifuser_b200.h: arena layout)

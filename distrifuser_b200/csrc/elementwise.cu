@@ -25,7 +25,6 @@ __device__ __forceinline__ float gelu_erf(float x) {
 __global__ void __launch_bounds__(256) geglu_kernel(const __half* __restrict__ in, __half* __restrict__ out, int64_t rows,
                                                     int vec_per_row, int64_t in_pitch, int64_t out_pitch, int cols) {
   const int64_t total = rows * vec_per_row;
-  pdl_wait();
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
     const int64_t r = i / vec_per_row;
     const int q = (int)(i - r * vec_per_row);
@@ -53,8 +52,9 @@ extern "C" int df_geglu(const void* in, void* out, int64_t rows, int cols, int64
   const int64_t total = rows * (cols / 8);
   int64_t g = (total + 255) / 256;
   if (g > kSmCount * 16) g = kSmCount * 16;
-  DF_CHECK_CUDA(launch_pdl(PDL_ELEM, geglu_kernel, dim3((unsigned)g), dim3(256), 0, (cudaStream_t)stream, (const __half*)in, (__half*)out, rows,
-                           cols / 8, in_pitch, out_pitch, cols));
+  geglu_kernel<<<(unsigned)g, 256, 0, (cudaStream_t)stream>>>((const __half*)in, (__half*)out, rows, cols / 8, in_pitch,
+                                                               out_pitch, cols);
+  DF_CHECK_LAUNCH();
   return 0;
 }
 
@@ -67,7 +67,6 @@ namespace {
 __global__ void __launch_bounds__(256) bias_residual_add_kernel(const __half* __restrict__ a, const __half* __restrict__ r,
                                                                 const __half* __restrict__ bias, __half* __restrict__ out,
                                                                 int64_t total_vec, int vec_per_row) {
-  pdl_wait();
   constexpr int U = 4;
   const int64_t stride = (int64_t)gridDim.x * blockDim.x;
   for (int64_t i0 = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i0 < total_vec; i0 += U * stride) {
@@ -113,8 +112,9 @@ extern "C" int df_bias_residual_add(const void* a, const void* residual, const v
   const int64_t total = rows * (C / 8);
   int64_t g = (total + 256 * 4 - 1) / (256 * 4);
   if (g > kSmCount * 8) g = kSmCount * 8;
-  DF_CHECK_CUDA(launch_pdl(PDL_ELEM, bias_residual_add_kernel, dim3((unsigned)g), dim3(256), 0, (cudaStream_t)stream, (const __half*)a,
-                           (const __half*)residual, (const __half*)bias, (__half*)out, total, C / 8));
+  bias_residual_add_kernel<<<(unsigned)g, 256, 0, (cudaStream_t)stream>>>((const __half*)a, (const __half*)residual,
+                                                                           (const __half*)bias, (__half*)out, total, C / 8);
+  DF_CHECK_LAUNCH();
   return 0;
 }
 
@@ -131,7 +131,6 @@ __global__ void __launch_bounds__(256) add_layernorm_kernel(const __half* __rest
                                                             int64_t rows, int C, float eps) {
   const int lane = threadIdx.x & 31;
   const int64_t row = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
-  pdl_wait();
   if (row >= rows) return;
   const int nvec = C >> 3;
   const __half* xr = x + row * C;
@@ -212,8 +211,8 @@ extern "C" int df_add_layernorm(const void* x, const void* r, void* s_out, void*
   const unsigned grid = (unsigned)((rows + warps - 1) / warps);
   cudaStream_t st = (cudaStream_t)stream;
   const int nvec = C / 8;
-#define DF_LN(MV) DF_CHECK_CUDA(launch_pdl(PDL_ELEM, add_layernorm_kernel<MV>, dim3(grid), dim3(warps * 32), 0, st, (const __half*)x, (const __half*)r, \
-      (__half*)s_out, (__half*)y, (const __half*)gamma, (const __half*)beta, rows, C, eps))
+#define DF_LN(MV) add_layernorm_kernel<MV><<<grid, warps * 32, 0, st>>>((const __half*)x, (const __half*)r, (__half*)s_out, \
+      (__half*)y, (const __half*)gamma, (const __half*)beta, rows, C, eps)
   if (nvec <= 32 * 2) DF_LN(2); else if (nvec <= 32 * 3) DF_LN(3); else if (nvec <= 32 * 5) DF_LN(5); else DF_LN(8);
 #undef DF_LN
   DF_CHECK_LAUNCH();

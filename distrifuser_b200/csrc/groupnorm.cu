@@ -361,7 +361,6 @@ __global__ void __launch_bounds__(512, 2) gn_fused_kernel(const __half* __restri
   extern __shared__ float2 ch[];                         // [lanes][C] moments; after the fold: red[G*tpp] | mine[G] | coef[G]
   __shared__ unsigned int my_gen;
   __shared__ bool is_last;
-  pdl_wait();
   GN_TR(0, blockIdx.x == 0 && blockIdx.y == 0 && threadIdx.x == 0);
   if (threadIdx.x == 0) my_gen = ld_volatile_u32(gen);   // read before this CTA's ticket: the bump needs every CTA's ticket
   __syncthreads();
@@ -494,9 +493,10 @@ int groupnorm_impl(df_comm_t comm, const void* x, const void* addend, int64_t ad
              p.nchunk * b, gn_resident_ctas());
   DF_REQUIRE(smem <= (size_t)kGnMaxSmem, "df_groupnorm_fwd: %zu bytes of shared memory exceed %d", smem, kGnMaxSmem);
   unsigned int* gen = ticket + 1;
-  DF_CHECK_CUDA(launch_pdl(PDL_GN, gn_fused_kernel, dim3(p.nchunk, b), dim3(p.threads), smem, st, (const __half*)x, (const __half*)addend, addend_pitch,
-                           (__half*)y, (const __half*)gamma, (const __half*)beta, partial, hw, C, groups, p.V,
-                           p.lanes, p.ppc, fuse_silu, ex, gen, halo));
+  gn_fused_kernel<<<dim3(p.nchunk, b), p.threads, smem, st>>>((const __half*)x, (const __half*)addend, addend_pitch, (__half*)y,
+                                                              (const __half*)gamma, (const __half*)beta, partial, hw, C, groups,
+                                                              p.V, p.lanes, p.ppc, fuse_silu, ex, gen, halo);
+  DF_CHECK_LAUNCH();
   return 0;
 }
 }  // namespace

@@ -102,7 +102,6 @@ linear_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant__ 
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
-  pdl_wait();                                              // set-up above overlapped the tail of the previous kernel
 
   if (warp == NCONSUMER_WARPS) {
     // =============================================================== TMA producer
@@ -220,7 +219,8 @@ int launch_linear(const CUtensorMap& ta, const CUtensorMap& tw, const LinearArgs
     DF_CHECK_CUDA(cudaFuncSetAttribute(linear_kernel<EPI, BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(SmemT<BN>)));
     attr_set = true;
   }
-  DF_CHECK_CUDA(launch_pdl(PDL_GEMM, linear_kernel<EPI, BN>, dim3(ctas), dim3(NTHREADS), sizeof(SmemT<BN>), st, ta, tw, args));
+  linear_kernel<EPI, BN><<<ctas, NTHREADS, sizeof(SmemT<BN>), st>>>(ta, tw, args);
+  DF_CHECK_LAUNCH();
   return 0;
 }
 

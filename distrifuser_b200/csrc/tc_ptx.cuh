@@ -19,9 +19,7 @@ __device__ __forceinline__ void mbar_arrive(uint32_t bar_addr) {      // by shar
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar_addr) : "memory");
 }
 __device__ __forceinline__ void mbar_arrive(uint64_t* bar) { mbar_arrive(smem_u32(bar)); }
-#ifndef DF_TRYWAIT_HINT_NS
-#define DF_TRYWAIT_HINT_NS 200000u
-#endif
+constexpr uint32_t kTryWaitHintNs = 200000u;
 __device__ __forceinline__ bool mbar_try(uint32_t bar_addr, uint32_t parity) {
   uint32_t ok;
   asm volatile(
@@ -29,12 +27,12 @@ __device__ __forceinline__ bool mbar_try(uint32_t bar_addr, uint32_t parity) {
       "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2, %3;\n\t"   // %3: suspend-time hint (ns): sleep in hardware,
       "selp.u32 %0, 1, 0, p;\n\t}"                                        // polling steals issue slots from the softmax warps
       : "=r"(ok)
-      : "r"(bar_addr), "r"(parity), "r"(DF_TRYWAIT_HINT_NS)
+      : "r"(bar_addr), "r"(parity), "r"(kTryWaitHintNs)
       : "memory");
   return ok != 0;
 }
 __device__ __forceinline__ bool mbar_try(uint64_t* bar, uint32_t parity) { return mbar_try(smem_u32(bar), parity); }
-// Waits for the phase with the given parity.  try_wait suspends the thread in hardware for up to DF_TRYWAIT_HINT_NS, so the loop
+// Waits for the phase with the given parity.  try_wait suspends the thread in hardware for up to kTryWaitHintNs, so the loop
 // costs two instructions per poll.  A broken pipeline still becomes a CUDA error instead of a hung GPU: after ~10 s of failed
 // polls the thread traps (define DF_MBAR_DEBUG for a printf naming the barrier).
 __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {

@@ -5,7 +5,6 @@ the reference's torch.cat of the per-rank K/V (attn.py:131-138), split / view / 
 F.scaled_dot_product_attention (:153) -- is one wgmma kernel (df_attn_fwd) that TMA-loads the K/V tiles
 straight from the n per-rank segments: this rank's fresh projection and the peers' 1-step-stale arena slots."""
 import ctypes as C
-import os
 
 import torch
 from torch import nn
@@ -138,7 +137,7 @@ class DistriSelfAttentionPP(DistriAttentionPP):
         LoRA fuse/unfuse, in-place edits, .to()/.half()): the key holds the tensors' version counters and storage.
         Heads narrower than 64 (SD1.x level 0: d = 40) are stored 64 wide -- zero rows in the projection, zero columns in
         to_out, the softmax scale passed explicitly: an 80-byte head row at offset 80*h of the token row costs the TMA 1.6 cache
-        lines per row request and leaves the kernel waiting for K/V tiles; 128-byte rows are one line each.  DF_PAD_HEADS=0 keeps the narrow layout."""
+        lines per row request and leaves the kernel waiting for K/V tiles; 128-byte rows are one line each."""
         to_q, to_kv = self.module.to_q, self.to_kv
         if not (isinstance(to_q, nn.Linear) and to_q.bias is None and to_kv.bias is None and
                 to_q.in_features == to_kv.in_features and to_q.out_features * 2 == to_kv.out_features and
@@ -147,7 +146,7 @@ class DistriSelfAttentionPP(DistriAttentionPP):
         wq, wkv, wo = to_q.weight, to_kv.weight, self.module.to_out[0].weight
         heads = self.module.heads
         d = to_q.out_features // heads
-        pad = 64 if (d < 64 and os.environ.get("DF_PAD_HEADS", "1") != "0") else 0
+        pad = 64 if d < 64 else 0
         key = (wq._version, wkv._version, wo._version, wq.data_ptr(), wkv.data_ptr(), wo.data_ptr(), wq.device, dtype, pad)
         if key != self._w_qkv_key:
             if torch.cuda.is_current_stream_capturing():

@@ -4,8 +4,6 @@ The halo rows go to the two patch neighbours only (df_halo_push, peer stores ove
 all_gather over every rank, and the padded conv input is assembled by one vectorised kernel
 (df_halo_assemble) instead of torch.stack + cat + F.pad.  The convolution itself stays a cuDNN library call
 on the NHWC padded tensor (SURVEY 8f N1 lists the hand-written implicit GEMM as a later row)."""
-import os
-
 import torch
 from torch import nn
 from torch.nn import functional as F
@@ -48,7 +46,7 @@ class DistriConv2dPP(BaseModule):
         the current call, else None (one patch, first layer, buffers not created yet, not 3x3 / padding 1)."""
         cfg = self.distri_config
         n = cfg.n_device_per_batch
-        if n == 1 or self.is_first_layer or not self._bound() or os.environ.get("DF_FUSED_HALO", "1") == "0":
+        if n == 1 or self.is_first_layer or not self._bound():
             return None
         m = self.module
         if m.padding[0] != 1 or m.kernel_size[0] != 3 or m.padding[1] != 1:

@@ -35,11 +35,6 @@ def add_layernorm(x: torch.Tensor, r: torch.Tensor | None, norm: torch.nn.LayerN
     return s, y
 
 
-def fused_conv_bias() -> bool:
-    """DF_CONV_BIAS=torch restores F.conv2d's own bias handling (cudnn_convolution + broadcast add_)."""
-    return _os.environ.get("DF_CONV_BIAS", "fused") != "torch"
-
-
 def conv2d_bias_residual(x: torch.Tensor, conv: torch.nn.Conv2d, padding, residual: torch.Tensor | None = None,
                          bias: torch.Tensor | None = None, fold_bias: bool = False) -> torch.Tensor:
     """conv(x) + bias (+ residual): the convolution runs in cuDNN WITHOUT bias and one vectorised pass adds `bias` (default
@@ -47,7 +42,7 @@ def conv2d_bias_residual(x: torch.Tensor, conv: torch.nn.Conv2d, padding, residu
     the following GroupNorm) -- no pass at all.  Falls back to F.conv2d for anything but fp16 CUDA NHWC tensors."""
     import torch.nn.functional as F
     b = conv.bias if bias is None else bias
-    ok = (x.is_cuda and x.dtype == torch.float16 and fused_conv_bias() and conv.out_channels % 8 == 0 and
+    ok = (x.is_cuda and x.dtype == torch.float16 and conv.out_channels % 8 == 0 and
           x.is_contiguous(memory_format=torch.channels_last))
     if not ok:
         out = F.conv2d(x, conv.weight, None if fold_bias else b, stride=conv.stride, padding=padding)

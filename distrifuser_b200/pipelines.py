@@ -5,8 +5,6 @@
 `from_pretrained` uses the real diffusers pipelines when the package (and weights) are available.  This image has
 neither, so `from_synthetic` builds the same object around a random-weight UNet of the SDXL / SD1.x architecture
 and a latent-space pipeline stand-in (compat/pipeline.py): that is what bench.py and the parity tests drive."""
-import os
-
 import torch
 
 from .models.distri_sdxl_unet_pp import DistriUNetPP
@@ -90,14 +88,13 @@ class _DistriPipelineBase:
             pool = None
             from . import _lib
             launches = []
-            # the compute kernels are captured on a stream of priority DF_COMPUTE_PRIO (default -1 = above the publication
-            # stream's 0): when a K/V projection finishes, the attention grid that follows it takes the SM slots before the
-            # publication kernel of the same K/V does -- a publication CTA that got there first keeps a persistent attention
-            # CTA out of its SM for the whole transfer
-            # no publications without patch peers (one patch, or naive patch)
+            # with patch peers the compute kernels are captured on a stream of priority -1 (above the publication stream's 0):
+            # when a K/V projection finishes, the attention grid that follows it takes the SM slots before the publication
+            # kernel of the same K/V does -- a publication CTA that got there first keeps a persistent attention CTA out of its
+            # SM for the whole transfer
+            # no publications without patch peers (one patch, or naive patch): priority 0
             patch_peers = cfg.parallelism == "patch" and cfg.n_device_per_batch > 1
-            prio = int(os.environ.get("DF_COMPUTE_PRIO", "-1" if patch_peers else "0"))
-            capture_stream = torch.cuda.Stream(device=cfg.device, priority=prio)
+            capture_stream = torch.cuda.Stream(device=cfg.device, priority=-1 if patch_peers else 0)
             for counter in unet.graph_counters():
                 graph = torch.cuda.CUDAGraph()
                 n0 = _lib.LAUNCHES["total"]

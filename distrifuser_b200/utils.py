@@ -300,8 +300,8 @@ class PatchParallelismCommManager:
         w.spin_timeout_ns = timeout_ns
         self.group, self.world, self.bank_stride = g, w, bank_stride
         # publication stream: the asynchronous K/V transfers have a whole denoise step of slack, so they must not pre-empt the
-        # compute kernels' CTA scheduling (DF_COMM_PRIO=-1 restores the high priority of round 1)
-        self.comm_stream = torch.cuda.Stream(device=cfg.device, priority=int(os.environ.get("DF_COMM_PRIO", "0")))
+        # compute kernels' CTA scheduling
+        self.comm_stream = torch.cuda.Stream(device=cfg.device, priority=0)
         import atexit
         import weakref
         ref = weakref.ref(self)
@@ -365,7 +365,7 @@ class PatchParallelismCommManager:
         if num_ctas is None:
             # synchronous steps wait for the data right away: use the whole NVLink; asynchronous publication hides under the
             # attention that follows and should take few SM slots
-            num_ctas = int(os.environ.get("DF_PUB_CTAS", "64")) if async_stream else 2 * 132   # two CTAs per SM of an H100
+            num_ctas = 64 if async_stream else 2 * 132   # two CTAs per SM of an H100
         main = torch.cuda.current_stream()
         if async_stream:
             self.comm_stream.wait_stream(main)      # fork: publication overlaps the compute that follows

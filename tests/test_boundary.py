@@ -55,6 +55,27 @@ def test_product_never_imports_oracle():
                 assert "/root/reference" not in text, f"{f} reads the reference tree"
 
 
+def test_no_code_path_switches():
+    """Environment variables may only observe the product (NVTX ranges, the flag-wait timeout, which library build to load)
+    or pick the Linears on the hand-written GEMM; none selects another code path, launch or tuning constant.  The CUDA sources
+    read no environment and take no tuning constant from a -D flag."""
+    import ast
+    allowed = {"DF_LIB_PATH", "DF_NVCC_FLAGS", "DF_NVTX", "DF_SPIN_TIMEOUT_S", "DF_LINEAR"}
+    found = set()
+    for dirpath, _, files in os.walk(os.path.join(ROOT, "distrifuser_b200")):
+        for f in files:
+            if f.endswith(".py"):
+                tree = ast.parse(open(os.path.join(dirpath, f)).read())
+                found |= {n.value for n in ast.walk(tree) if isinstance(n, ast.Constant) and isinstance(n.value, str)
+                          and re.fullmatch(r"DF_[A-Z0-9_]+", n.value)}
+    assert "DF_LINEAR" in found and found <= allowed, f"environment switches outside the allowed set: {sorted(found - allowed)}"
+    csrc = os.path.join(ROOT, "distrifuser_b200", "csrc")
+    for f in os.listdir(csrc):
+        text = open(os.path.join(csrc, f)).read()
+        assert "getenv(" not in text, f"{f} reads the environment"
+        assert not re.search(r"#\s*ifndef\s+DF_", text), f"{f} takes a tuning constant from a -D flag"
+
+
 def test_api_surface_matches_reference_names():
     from distrifuser_b200.models.distri_sdxl_unet_pp import DistriUNetPP
     from distrifuser_b200.modules.base_module import BaseModule

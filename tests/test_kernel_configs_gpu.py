@@ -2,13 +2,10 @@
 over several peer segments (the 8-GPU plans of SD1.5 / SDXL at 1024^2), the strided q | k | v views of the fused projection,
 zero-padded heads with an explicit softmax scale, every head width of the NBLK blocks; GroupNorm exchange modes inside an
 asynchronous step, the negative-variance fallback, the fused halo with statistics exchange and edge shapes; the output gather
-and the epoch clock; the GEMM's forced tile widths, CTA caps, pitched output / residual and fused publication; programmatic
-dependent launch.  References are fp32 (fp64 where noted) torch restatements of the same math; tolerances as in
-test_kernels_gpu.py / test_linear_gpu.py.  Every test first asserts that it reaches the path it is about."""
+and the epoch clock; the GEMM's forced tile widths, CTA caps, pitched output / residual and fused publication.  References
+are fp32 (fp64 where noted) torch restatements of the same math; tolerances as in test_kernels_gpu.py / test_linear_gpu.py.
+Every test first asserts that it reaches the path it is about."""
 import ctypes as C
-import os
-import subprocess
-import sys
 
 import pytest
 import torch
@@ -638,24 +635,3 @@ def test_linear_minimal_shape():
     r = torch.randn(M, N, device="cuda").half()
     out = _linear(x, w, torch.empty(M, N, device="cuda", dtype=torch.float16), bias=b, residual=r)
     _close(out, (x.float() @ w.float().t() + b.float()).half().float() + r.float())
-
-
-# ================================================================================================================ PDL
-def test_pdl_chain_bit_identical(tmp_path):
-    """The seeded kernel chain of pdl_chain.py with programmatic dependent launch on for every kernel family (DF_PDL=15) and
-    off: every output bit-identical (all kernels involved are deterministic by construction)."""
-    script = os.path.join(os.path.dirname(os.path.abspath(__file__)), "pdl_chain.py")
-    got = []
-    for pdl in ("15", None):
-        env = {k: v for k, v in os.environ.items() if k != "DF_PDL"}
-        if pdl:
-            env["DF_PDL"] = pdl
-        path = tmp_path / f"pdl_{pdl or 'off'}.pt"
-        cmd = [sys.executable] + (["-s"] if sys.flags.no_user_site else []) + [script, str(path)]
-        r = subprocess.run(cmd, env=env, capture_output=True, text=True, timeout=600)
-        assert r.returncode == 0, f"DF_PDL={pdl}: {r.stdout}\n{r.stderr}"
-        got.append(torch.load(path))
-    on, off = got
-    assert on["pdl"] == 15 and off["pdl"] == 0 and on["out"].keys() == off["out"].keys()
-    for k in on["out"]:
-        assert torch.equal(on["out"][k], off["out"][k]), f"{k} differs with DF_PDL=15"
