@@ -70,10 +70,16 @@ class DistriConfig:
             rank, world_size = dist.get_rank(), dist.get_world_size()
         else:
             rank, world_size = 0, 1                                     # utils.py:44-47 (single GPU)
-        assert is_power_of_2(world_size)                                # utils.py:49
-        assert world_size <= _lib.MAX_WORLD, (
+        # any GPU count of one box: the reference asserts a power of two (utils.py:49), but row strips need not be equal here
+        # (split_units) and every communicator kernel takes a member count and mask up to DF_MAX_WORLD
+        assert 1 <= world_size <= _lib.MAX_WORLD, (
             f"distrifuser_b200 shards one image over the GPUs of ONE NVSwitch box (<= {_lib.MAX_WORLD} ranks, "
             f"DF_MAX_WORLD); got world_size={world_size}")
+        if do_classifier_free_guidance and split_batch and world_size > 1 and world_size % 2:
+            # two CFG groups of unequal size would leave the larger one's latency for the whole step
+            raise ValueError(f"split_batch=True splits the CFG batch into two patch groups of world_size / 2 ranks; "
+                             f"world_size={world_size} is odd: pass split_batch=False, which runs both CFG branches on "
+                             f"every rank over {world_size} patches")
         assert mode in ("corrected_async_gn", "stale_gn", "sync_gn", "separate_gn", "full_sync", "no_sync")
         if parallelism == "naive_patch":
             if split_scheme not in ("row", "col", "alternate"):                 # NaivePatchUNet.forward raises the same

@@ -8,6 +8,12 @@ on all of them alike.  Prints one JSON line with the card name and power limit b
     python -m torch.distributed.run --nproc-per-node N tools/bench_parallelism.py [--rounds 3] [--images 2] [--resolution 1024]
         [--dump-outputs DIR]      # rank 0 writes each configuration's final latents to DIR/<config>.npy
 
+Any N from 1 to 8.  An odd N runs both CFG branches on every rank (split_batch=False: two CFG groups need an even N); an even
+N splits the CFG batch unless --no-split-batch.  Naive patch needs strips of whole latent rows / columns: a configuration
+that does not cut into them at the chosen resolution is skipped and the reason recorded.  At --resolution 1536 (192 latent
+rows, 48 SDXL row units) every configuration runs at N in {1, 2, 3, 4, 6, 8}; at 1024 naive patch runs at N in {1, 2, 4, 8}
+only, and at N = 5 or 7 only patch parallelism runs at either resolution.
+
 One GPU per rank: with fewer GPUs than ranks the ranks would time-slice one device, so the script then times nothing and
 reports "not measured"."""
 from __future__ import annotations
@@ -66,10 +72,17 @@ def main():
     from distrifuser_b200.utils import DistriConfig
 
     R = a.resolution
-    pipes = {}
+    split = not a.no_split_batch and world % 2 == 0
+    pipes, skipped = {}, {}
     for par, scheme in CONFIGS:
         name = par if par == "patch" else f"naive_{scheme}"
-        cfg = DistriConfig(height=R, width=R, split_batch=not a.no_split_batch, parallelism=par, split_scheme=scheme)
+        try:
+            cfg = DistriConfig(height=R, width=R, split_batch=split, parallelism=par, split_scheme=scheme)
+        except ValueError as e:                                      # naive strips that are not whole latent rows / columns
+            if par != "naive_patch":
+                raise
+            skipped[name] = str(e)
+            continue
         pipe = DistriSDXLPipeline.from_synthetic(cfg, seed=0)
         pipe.set_progress_bar_config(disable=True)
         pipes[name] = pipe
@@ -110,9 +123,10 @@ def main():
     if rank == 0:
         print(json.dumps({
             "bench": "parallelism", "workload": f"synthetic SDXL {R}x{R}, {bench.STEPS_PER_IMAGE} Euler steps, CFG, CUDA graphs",
-            "world_size": world, "split_batch": not a.no_split_batch, "card": gpu,
+            "world_size": world, "split_batch": split, "card": gpu,
             "ms_per_image": {k: round(statistics.median(v), 1) for k, v in times.items()},
             "ms_per_image_rounds": {k: [round(x, 1) for x in v] for k, v in times.items()},
+            "skipped": skipped,
         }), flush=True)
     barrier()
     for pipe in pipes.values():
