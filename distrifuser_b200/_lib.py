@@ -13,6 +13,7 @@ NBANKS = 3
 MAX_WORLD = 8
 IPC_HANDLE_BYTES = 64
 TENSORMAP_BYTES = 128
+ZERO_CONV_MAX_PROBLEMS = 13
 
 EXPORTS = (
     "df_last_error", "df_version", "df_device_sm_count", "df_symm_alloc", "df_symm_open", "df_symm_close",
@@ -21,6 +22,7 @@ EXPORTS = (
     "df_halo_assemble", "df_attn_make_kvmaps", "df_attn_workspace_bytes", "df_attn_fwd", "df_attn_make_kvmaps_ragged",
     "df_attn_workspace_bytes_ragged", "df_attn_fwd_ragged",
     "df_output_gather", "df_output_gather_2d", "df_geglu", "df_add_layernorm", "df_bias_residual_add", "df_linear_supported", "df_linear_geglu_block", "df_linear_fwd",
+    "df_controlnet_zero_convs",
 )
 
 
@@ -82,6 +84,8 @@ def lib():
         L.df_linear_geglu_block.argtypes = [i64, i32, i32]
         L.df_linear_fwd.argtypes = [DfComm, vp, vp, vp, vp, vp, i64, i32, i32, i64, i64, i64, i64, i32, i32, i32, i32, i32, u32, u64,
                                     u64, i32, vp]
+        L.df_controlnet_zero_convs.argtypes = [i32, C.POINTER(vp), C.POINTER(vp), C.POINTER(vp), C.POINTER(vp),
+                                               C.POINTER(i64), C.POINTER(C.c_int32), C.POINTER(C.c_int32), vp, i32, vp]
         L.df_output_gather.argtypes = [DfComm, vp, vp, i32, i32, i32, i32, i32, i32, i32, i32, i32, u64, vp]
         L.df_output_gather_2d.argtypes = [DfComm, vp, vp, i32, i32, i32, i32, i32, i32, i32, i32, i32, i32, i32, u64, vp]
         for name in EXPORTS:
@@ -94,7 +98,7 @@ def lib():
 KERNELS_PER_CALL = {"df_groupnorm_fwd": 1, "df_groupnorm_halo_fwd": 1, "df_attn_fwd": 1, "df_groupnorm_fwd_weighted": 1,
                     "df_groupnorm_halo_fwd_weighted": 1, "df_attn_fwd_ragged": 1, "df_halo_push": 1, "df_halo_assemble": 1,
                     "df_slot_publish": 1, "df_slot_wait": 1, "df_step_begin": 1, "df_output_gather": 2, "df_output_gather_2d": 2, "df_geglu": 1, "df_add_layernorm": 1, "df_bias_residual_add": 1,
-                    "df_linear_fwd": 1}
+                    "df_linear_fwd": 1, "df_controlnet_zero_convs": 1}
 LAUNCHES = {"total": 0}
 PROFILE = None   # bench.py sets this to a list; kernels then bracket their launch with CUDA events on the launching stream
 

@@ -53,7 +53,9 @@ class SyntheticLatentPipeline:
 
     @torch.no_grad()
     def __call__(self, prompt="", height=1024, width=1024, num_inference_steps=50, guidance_scale=5.0, generator=None,
-                 latents=None, output_type="latent", prompt_embeds=None, pooled_prompt_embeds=None, **kwargs):
+                 latents=None, output_type="latent", prompt_embeds=None, pooled_prompt_embeds=None, image=None,
+                 controlnet_conditioning_scale=1.0, **kwargs):
+        """image: the ControlNet conditioning image [1, 3, height, width] when the UNet has a ControlNet attached."""
         dev = self.device
         cfg_on = guidance_scale > 1.0
         if prompt_embeds is None:
@@ -77,11 +79,17 @@ class SyntheticLatentPipeline:
         if self.sdxl:
             ids = self._get_add_time_ids((height, width), (0, 0), (height, width), self.dtype).to(dev).repeat(B, 1)
             added = {"text_embeds": pooled_prompt_embeds, "time_ids": ids}
+        control = {}
+        if image is not None:                                        # both CFG branches get the same conditioning image
+            cond = image.to(dev, self.dtype)
+            control = dict(controlnet_cond=torch.cat([cond] * 2) if cfg_on else cond,
+                           conditioning_scale=controlnet_conditioning_scale)
         for i in range(num_inference_steps):
             t = self.scheduler.timesteps[i]
             x = torch.cat([lat] * 2) if cfg_on else lat
             x = self.scheduler.scale_model_input(x, t).to(self.dtype)
-            eps = self.unet(x, t, encoder_hidden_states=prompt_embeds, added_cond_kwargs=added, return_dict=False)[0]
+            eps = self.unet(x, t, encoder_hidden_states=prompt_embeds, added_cond_kwargs=added, return_dict=False,
+                            **control)[0]
             if cfg_on:
                 e_u, e_c = eps.float().chunk(2)
                 eps = e_u + guidance_scale * (e_c - e_u)

@@ -444,7 +444,11 @@ class UNet2DConditionModel(nn.Module):
         for blk in self.down_blocks:
             x, s = blk(x, emb, encoder_hidden_states)
             skips += s
+        if down_block_additional_residuals is not None:              # ControlNet: skip i + residual i, as diffusers adds them
+            skips = [s + r for s, r in zip(skips, down_block_additional_residuals, strict=True)]
         x = self.mid_block(x, emb, encoder_hidden_states)
+        if mid_block_additional_residual is not None:
+            x = x + mid_block_additional_residual
         for blk in self.up_blocks:
             x = blk(x, skips, emb, encoder_hidden_states)
         if self.fused_norm_act and hasattr(self.conv_out, "halo_plan") and self.conv_out.halo_plan(x) is not None:

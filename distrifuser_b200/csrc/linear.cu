@@ -83,12 +83,52 @@ __device__ __forceinline__ void wgmma_tile(float* acc, uint64_t a_desc, uint64_t
   else wgmma_ss_n160(acc, a_desc, b_desc, accumulate);
 }
 
+// The mainloop, shared by every GEMM kernel of this file.  Producer (one lane): TMA-loads the K blocks of the 128 x BN tile
+// (tm, tn) into the stage ring.  Consumers (both warpgroups): acc = A tile . W tile^T over those K blocks, each stage released
+// once the wgmmas that read it have retired.  Producer and consumers walk the same tile sequence, so the ring stays in step.
+template <int BN>
+__device__ __forceinline__ void load_tile(SmemT<BN>& sm, const void* tm_a, const void* tm_w, int tm, int tn, int kblocks,
+                                          uint32_t& stage, uint32_t& phase) {
+  constexpr int STAGES = Stages<BN>::value;
+  constexpr uint32_t B_BYTES = BN * BK * 2;
+  for (int kb = 0; kb < kblocks; ++kb) {
+    mbar_wait(&sm.empty[stage], phase ^ 1u);
+    mbar_expect_tx(&sm.full[stage], A_BYTES + B_BYTES);
+    tma_load_2d(sm.a[stage], tm_a, &sm.full[stage], kb * BK, tm * BM);
+    tma_load_2d(sm.b[stage], tm_w, &sm.full[stage], kb * BK, tn * BN);
+    if (++stage == STAGES) { stage = 0; phase ^= 1u; }
+  }
+}
+
+template <int BN>
+__device__ __forceinline__ void mma_tile(SmemT<BN>& sm, float* acc, int wg, int lane, int kblocks, uint32_t& stage,
+                                         uint32_t& phase) {
+  constexpr int STAGES = Stages<BN>::value;
+  fence_regs<BN / 2>(acc);
+  uint32_t prev = 0;
+  for (int kb = 0; kb < kblocks; ++kb) {
+    mbar_wait(&sm.full[stage], phase);
+    const uint32_t a_addr = smem_u32(sm.a[stage]) + wg * 64 * 128, b_addr = smem_u32(sm.b[stage]);
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < BK / 16; ++kk)
+      wgmma_tile<BN>(acc, smem_desc(a_addr + kk * 32, 16, 1024), smem_desc(b_addr + kk * 32, 16, 1024), (kb | kk) > 0);
+    wgmma_commit();
+    wgmma_wait<1>();                                   // the previous K block's wgmmas have retired: its stage is free
+    if (kb > 0 && lane == 0) mbar_arrive(&sm.empty[prev]);
+    prev = stage;
+    if (++stage == STAGES) { stage = 0; phase ^= 1u; }
+  }
+  wgmma_wait<0>();
+  fence_regs<BN / 2>(acc);
+  if (lane == 0) mbar_arrive(&sm.empty[prev]);
+}
+
 template <int EPI, int BN>
 __global__ void __launch_bounds__(NTHREADS, 1)
 linear_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant__ CUtensorMap tm_w, LinearArgs p) {
   static_assert(BN % 32 == 0 && BN <= 256 && (BN * BK * 2) % 1024 == 0, "tile shape");
   constexpr int STAGES = Stages<BN>::value;
-  constexpr uint32_t B_BYTES = BN * BK * 2;
   using Smem = SmemT<BN>;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   Smem& sm = *reinterpret_cast<Smem*>(smem_raw);
@@ -109,16 +149,8 @@ linear_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant__ 
       prefetch_tmap(&tm_a);
       prefetch_tmap(&tm_w);
       uint32_t stage = 0, phase = 0;
-      for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
-        const int tm = tile % p.tiles_m, tn = tile / p.tiles_m;
-        for (int kb = 0; kb < kblocks; ++kb) {
-          mbar_wait(&sm.empty[stage], phase ^ 1u);
-          mbar_expect_tx(&sm.full[stage], A_BYTES + B_BYTES);
-          tma_load_2d(sm.a[stage], &tm_a, &sm.full[stage], kb * BK, tm * BM);
-          tma_load_2d(sm.b[stage], &tm_w, &sm.full[stage], kb * BK, tn * BN);
-          if (++stage == STAGES) { stage = 0; phase ^= 1u; }
-        }
-      }
+      for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x)
+        load_tile<BN>(sm, &tm_a, &tm_w, tile % p.tiles_m, tile / p.tiles_m, kblocks, stage, phase);
     }
   } else {
     // =============================================================== consumers (warps 0-7): main loop + epilogue
@@ -131,24 +163,7 @@ linear_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant__ 
     float acc[BN / 2];
     for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
       const int tm = tile % p.tiles_m, tn = tile / p.tiles_m;
-      fence_regs<BN / 2>(acc);
-      uint32_t prev = 0;
-      for (int kb = 0; kb < kblocks; ++kb) {
-        mbar_wait(&sm.full[stage], phase);
-        const uint32_t a_addr = smem_u32(sm.a[stage]) + wg * 64 * 128, b_addr = smem_u32(sm.b[stage]);
-        wgmma_fence();
-#pragma unroll
-        for (int kk = 0; kk < BK / 16; ++kk)
-          wgmma_tile<BN>(acc, smem_desc(a_addr + kk * 32, 16, 1024), smem_desc(b_addr + kk * 32, 16, 1024), (kb | kk) > 0);
-        wgmma_commit();
-        wgmma_wait<1>();                                   // the previous K block's wgmmas have retired: its stage is free
-        if (kb > 0 && lane == 0) mbar_arrive(&sm.empty[prev]);
-        prev = stage;
-        if (++stage == STAGES) { stage = 0; phase ^= 1u; }
-      }
-      wgmma_wait<0>();
-      fence_regs<BN / 2>(acc);
-      if (lane == 0) mbar_arrive(&sm.empty[prev]);
+      mma_tile<BN>(sm, acc, wg, lane, kblocks, stage, phase);
 #pragma unroll
       for (int h = 0; h < 2; ++h) {                        // accumulator rows A / B of this thread
         const int64_t grow = (int64_t)tm * BM + rloc + 8 * h;
@@ -304,4 +319,139 @@ extern "C" int df_linear_fwd(df_comm_t comm, const void* a, const void* w, const
   }
   if (bn == 160) return launch_linear<EPI_PLAIN, 160>(ta, tw, args, ctas, st);
   return launch_linear<EPI_PLAIN, 256>(ta, tw, args, ctas, st);
+}
+
+// ----------------------------------------------------------------------------------------- ControlNet zero convolutions
+// out_i[M_i, N_i] = scale * (x_i[M_i, K_i] . W_i[N_i, K_i]^T + b_i) for every 1x1 "zero" conv of one ControlNet call, in ONE
+// persistent launch of the mainloop above.  The problem list (tensor maps, bias / output pointers, tile offsets) is a
+// __grid_constant__ parameter: it lives in the kernel's parameter space on the device, so a captured CUDA graph carries it and
+// no host-to-device upload of a list is needed per call or per graph.  `scale` is read from device memory, so a replay of a
+// captured graph honours a new conditioning scale.  Tiles are 128 x 160: 160 divides every ControlNet width (320, 640, 1280).
+// K need only be a multiple of 8 (16-byte rows for TMA): the last K block's columns past K arrive as zeros in both operands.
+namespace {
+constexpr int ZC_BN = 160;
+
+struct ZeroConvProblem {
+  const __half* bias;       // [N] or null
+  __half* out;              // [M, N] contiguous
+  int M, N, tiles_m, tile0, kblocks;
+};
+
+struct ZeroConvArgs {
+  CUtensorMap a[DF_ZERO_CONV_MAX_PROBLEMS], w[DF_ZERO_CONV_MAX_PROBLEMS];
+  ZeroConvProblem p[DF_ZERO_CONV_MAX_PROBLEMS];
+  const float* scale;
+  int nproblems, ntiles;
+};
+static_assert(sizeof(ZeroConvArgs) <= 4096, "the problem list must fit the 4 KiB kernel parameter space");
+
+__device__ __forceinline__ int zc_problem(const ZeroConvArgs& z, int tile) {
+  int q = 0;
+  while (q + 1 < z.nproblems && tile >= z.p[q + 1].tile0) ++q;
+  return q;
+}
+
+__global__ void __launch_bounds__(NTHREADS, 1) zero_conv_kernel(const __grid_constant__ ZeroConvArgs z) {
+  constexpr int BN = ZC_BN;
+  constexpr int STAGES = Stages<BN>::value;
+  using Smem = SmemT<BN>;
+  extern __shared__ __align__(1024) uint8_t smem_raw[];
+  Smem& sm = *reinterpret_cast<Smem*>(smem_raw);
+  if ((smem_u32(smem_raw) & 1023u) != 0) __trap();
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < STAGES; ++s) { mbar_init(&sm.full[s], 1); mbar_init(&sm.empty[s], NCONSUMER_WARPS); }
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  __syncthreads();
+
+  if (warp == NCONSUMER_WARPS) {
+    if (lane == 0) {
+      uint32_t stage = 0, phase = 0;
+      for (int tile = blockIdx.x; tile < z.ntiles; tile += gridDim.x) {
+        const int q = zc_problem(z, tile);
+        const ZeroConvProblem& p = z.p[q];
+        const int t = tile - p.tile0;
+        load_tile<BN>(sm, &z.a[q], &z.w[q], t % p.tiles_m, t / p.tiles_m, p.kblocks, stage, phase);
+      }
+    }
+  } else {
+    const int wg = warp >> 2;
+    const int c4 = lane & 3;
+    const int rloc = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+    const float scale = *z.scale;
+    uint32_t stage = 0, phase = 0;
+    float acc[BN / 2];
+    for (int tile = blockIdx.x; tile < z.ntiles; tile += gridDim.x) {
+      const ZeroConvProblem& p = z.p[zc_problem(z, tile)];
+      const int t = tile - p.tile0;
+      const int tm = t % p.tiles_m, tn = t / p.tiles_m;
+      mma_tile<BN>(sm, acc, wg, lane, p.kblocks, stage, phase);
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int64_t grow = (int64_t)tm * BM + rloc + 8 * h;
+        if (grow >= p.M) continue;
+        const int col0 = tn * BN;
+        __half* dst = p.out + grow * p.N + col0;
+#pragma unroll
+        for (int i = 0; i < BN / 8; ++i) {
+          const int c = 8 * i + 2 * c4;
+          const int col = col0 + c;
+          if (col >= p.N) continue;                        // N % 8 == 0: a column pair is entirely inside or outside
+          float2 f = make_float2(acc[4 * i + 2 * h], acc[4 * i + 2 * h + 1]);
+          if (p.bias) { const float2 bb = ld_h2f(p.bias + col); f.x += bb.x; f.y += bb.y; }
+          // torch: the fp16 conv output, then the scale multiply in fp32 rounded to fp16
+          const float2 r = __half22float2(__floats2half2_rn(f.x, f.y));
+          *reinterpret_cast<__half2*>(dst + c) = __floats2half2_rn(r.x * scale, r.y * scale);
+        }
+      }
+    }
+  }
+}
+}  // namespace
+
+extern "C" int df_controlnet_zero_convs(int nproblems, const void* const* x_host, const void* const* w_host,
+                                        const void* const* bias_host, void* const* out_host, const int64_t* m_host,
+                                        const int32_t* n_host, const int32_t* k_host, const float* scale, int max_ctas,
+                                        void* stream) {
+  DF_REQUIRE(nproblems >= 1 && nproblems <= DF_ZERO_CONV_MAX_PROBLEMS, "df_controlnet_zero_convs: %d problems (1..%d)",
+             nproblems, DF_ZERO_CONV_MAX_PROBLEMS);
+  DF_REQUIRE(x_host && w_host && out_host && m_host && n_host && k_host && scale, "df_controlnet_zero_convs: null argument");
+  DF_REQUIRE(((uintptr_t)scale % 4) == 0, "df_controlnet_zero_convs: scale must be a 4-byte aligned fp32");
+  ZeroConvArgs z;
+  memset(&z, 0, sizeof(z));
+  int ntiles = 0;
+  for (int i = 0; i < nproblems; ++i) {
+    const int64_t M = m_host[i];
+    const int N = n_host[i], K = k_host[i];
+    const void* bias = bias_host ? bias_host[i] : nullptr;
+    DF_REQUIRE(M >= 1 && M <= INT32_MAX && N >= 8 && N % 8 == 0 && K >= 8 && K % 8 == 0,
+               "df_controlnet_zero_convs: problem %d has unsupported shape M=%lld N=%d K=%d (N %% 8, K %% 8)", i,
+               (long long)M, N, K);
+    DF_REQUIRE(x_host[i] && w_host[i] && out_host[i] && ((uintptr_t)x_host[i] % 16) == 0 &&
+                   ((uintptr_t)w_host[i] % 16) == 0 && ((uintptr_t)out_host[i] % 16) == 0 && ((uintptr_t)bias % 16) == 0,
+               "df_controlnet_zero_convs: problem %d: operands must be non-null and 16-byte aligned", i);
+    if (int rc = make_map2d(&z.a[i], x_host[i], M, K, K, BM)) return rc;
+    if (int rc = make_map2d(&z.w[i], w_host[i], N, K, K, ZC_BN)) return rc;
+    ZeroConvProblem& p = z.p[i];
+    p.bias = (const __half*)bias; p.out = (__half*)out_host[i];
+    p.M = (int)M; p.N = N; p.kblocks = (K + BK - 1) / BK;        // TMA zero-fills the columns past K of the last block
+    p.tiles_m = (int)((M + BM - 1) / BM);
+    p.tile0 = ntiles;
+    const int64_t t = (int64_t)p.tiles_m * ((N + ZC_BN - 1) / ZC_BN);
+    DF_REQUIRE(ntiles + t <= INT32_MAX, "df_controlnet_zero_convs: too many tiles");
+    ntiles += (int)t;
+  }
+  z.scale = scale; z.nproblems = nproblems; z.ntiles = ntiles;
+  const int cap = max_ctas > 0 ? max_ctas : sm_count();
+  const int ctas = ntiles < cap ? ntiles : cap;
+  static bool attr_set = false;
+  if (!attr_set) {
+    DF_CHECK_CUDA(cudaFuncSetAttribute(zero_conv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(SmemT<ZC_BN>)));
+    attr_set = true;
+  }
+  zero_conv_kernel<<<ctas, NTHREADS, sizeof(SmemT<ZC_BN>), (cudaStream_t)stream>>>(z);
+  DF_CHECK_LAUNCH();
+  return 0;
 }

@@ -38,7 +38,7 @@ def cfg_branch(cfg: DistriConfig, sample, timestep, encoder_hidden_states, added
     return sample, timestep, encoder_hidden_states, added_cond_kwargs
 
 
-def load_static_inputs(si: dict, sample, timestep, encoder_hidden_states, added_cond_kwargs) -> None:
+def load_static_inputs(si: dict, sample, timestep, encoder_hidden_states, added_cond_kwargs, controlnet_cond=None) -> None:
     """Copies a call's inputs into the captured graphs' static inputs (distri_sdxl_unet_pp.py:89-106)."""
     assert si["sample"].shape == sample.shape
     si["sample"].copy_(sample)
@@ -50,6 +50,8 @@ def load_static_inputs(si: dict, sample, timestep, encoder_hidden_states, added_
     if added_cond_kwargs is not None:
         for k in added_cond_kwargs:
             si["added_cond_kwargs"][k].copy_(added_cond_kwargs[k])
+    if controlnet_cond is not None and controlnet_cond is not si["controlnet_cond"]:
+        si["controlnet_cond"].copy_(controlnet_cond)
 
 
 class BaseModel(*_BASES):
@@ -69,6 +71,32 @@ class BaseModel(*_BASES):
         self.static_outputs = None
         self.cuda_graphs = None
         self.graph_launches = None       # number of this package's kernels inside each captured graph
+        self.controlnet = None           # DistriControlNetPP run inside forward() (DistriUNetPP only)
+        self._cn_scale = None            # device fp32 [1] set with the ControlNet: the scale the zero-conv kernel reads
+
+    def _wrapped_modules(self):
+        models = [self.model] if self.controlnet is None else [self.controlnet.model, self.model]
+        return [m for model in models for m in model.modules() if isinstance(m, BaseModule)]
+
+    def _controlnet_inputs(self, b, h, w, controlnet_cond, conditioning_scale):
+        """Checks the conditioning image against the latent and loads the scale into the device scalar the graphs read."""
+        if self.controlnet is None:
+            if controlnet_cond is not None:
+                raise ValueError("controlnet_cond was given but this UNet has no ControlNet attached (pass controlnet=... to "
+                                 "from_synthetic or DistriUNetPP)")
+            return None
+        if controlnet_cond is None:
+            raise ValueError("this UNet has a ControlNet attached: pass the conditioning image as controlnet_cond=[B, 3, H, W]")
+        want = (b, self.controlnet.model.controlnet_cond_embedding.conv_in.module.in_channels, 8 * h, 8 * w)
+        if tuple(controlnet_cond.shape) != want:
+            raise ValueError(f"controlnet_cond has shape {tuple(controlnet_cond.shape)}; the {b}x4x{h}x{w} latent needs the "
+                             f"conditioning image at pixel resolution, {want}")
+        if conditioning_scale is not self._cn_scale:                 # a graph capture passes the device scalar itself
+            if torch.is_tensor(conditioning_scale):
+                self._cn_scale.copy_(conditioning_scale.reshape(1))
+            else:
+                self._cn_scale.fill_(float(conditioning_scale))
+        return self._cn_scale
 
     def _strip(self, sample):
         """-> (UNet input of this rank, (row0, col0, hs, ws): the rows and columns of the image its output covers)."""
@@ -106,24 +134,34 @@ class BaseModel(*_BASES):
         mid_block_additional_residual=None,
         down_intrablock_additional_residuals=None,
         encoder_attention_mask=None,
+        controlnet_cond=None,
+        conditioning_scale=1.0,
         return_dict: bool = True,
         record: bool = False,
     ):
+        """`controlnet_cond` ([B, 3, H, W] fp16) and `conditioning_scale` (a float or a device scalar) are not diffusers
+        arguments: with a ControlNet attached, forward() runs it on this rank's strip and hands its residual strips to the UNet."""
         cfg = self.distri_config
         b, c, h, w = sample.shape
+        if down_block_additional_residuals is not None or mid_block_additional_residual is not None:
+            raise ValueError("residuals from outside cannot be used: each rank runs the UNet on its own strip, on one epoch per "
+                             "denoising step, and a ControlNet called separately would advance that clock twice per step; attach "
+                             "the ControlNet to the UNet (controlnet=...) and pass controlnet_cond=... instead")
         assert (class_labels is None and timestep_cond is None and attention_mask is None
-                and cross_attention_kwargs is None and down_block_additional_residuals is None
-                and mid_block_additional_residual is None and down_intrablock_additional_residuals is None
+                and cross_attention_kwargs is None and down_intrablock_additional_residuals is None
                 and encoder_attention_mask is None)                  # distri_sdxl_unet_pp.py:63-72
+        scale = self._controlnet_inputs(b, h, w, controlnet_cond, conditioning_scale)
         split = cfg.world_size > 1 and cfg.do_classifier_free_guidance and cfg.split_batch
         if split:
             assert b == 2
             sample, timestep, encoder_hidden_states, added_cond_kwargs = cfg_branch(
                 cfg, sample, timestep, encoder_hidden_states, added_cond_kwargs)
+            if controlnet_cond is not None:
+                controlnet_cond = controlnet_cond[cfg.batch_idx():cfg.batch_idx() + 1]
         B = 2 if split else b
 
         if cfg.use_cuda_graph and not record and self.cuda_graphs is not None:
-            load_static_inputs(self.static_inputs, sample, timestep, encoder_hidden_states, added_cond_kwargs)
+            load_static_inputs(self.static_inputs, sample, timestep, encoder_hidden_states, added_cond_kwargs, controlnet_cond)
             graph_idx = self._graph_idx()                            # distri_sdxl_unet_pp.py:108-113
             self.cuda_graphs[graph_idx].replay()
             if self.graph_launches is not None:
@@ -139,8 +177,15 @@ class BaseModel(*_BASES):
             # NHWC inside the UNet; `sample` itself stays the (sliced) view of the caller's tensor so that a captured
             # graph re-reads the static input on every replay
             x, (row0, col0, hs, ws) = self._strip(sample)
-            output = self.model(x.contiguous(memory_format=torch.channels_last), timestep, encoder_hidden_states,
-                                added_cond_kwargs=added_cond_kwargs, return_dict=False)[0]
+            x = x.contiguous(memory_format=torch.channels_last)
+            residuals = {}
+            if self.controlnet is not None:                          # ControlNet first: it registers and publishes first
+                down, mid = self.controlnet(x, timestep, encoder_hidden_states,
+                                            controlnet_cond.contiguous(memory_format=torch.channels_last), scale,
+                                            added_cond_kwargs=added_cond_kwargs)
+                residuals = dict(down_block_additional_residuals=down, mid_block_additional_residual=mid)
+            output = self.model(x, timestep, encoder_hidden_states, added_cond_kwargs=added_cond_kwargs, return_dict=False,
+                                **residuals)[0]
             if cfg.world_size > 1 and live:                          # distri_sdxl_unet_pp.py:162-169 / 186-193
                 # Every rank waits here for the strips of every world rank: the gather is a per-call world barrier, which
                 # is what keeps the output banks safe to reuse (BANK-REUSE INVARIANT in utils.py).
@@ -163,7 +208,8 @@ class BaseModel(*_BASES):
                 if self.static_inputs is None:                       # distri_sdxl_unet_pp.py:194-201
                     self.static_inputs = {"sample": sample, "timestep": timestep,
                                           "encoder_hidden_states": encoder_hidden_states,
-                                          "added_cond_kwargs": added_cond_kwargs}
+                                          "added_cond_kwargs": added_cond_kwargs, "controlnet_cond": controlnet_cond,
+                                          "conditioning_scale": scale}
                 self.synchronize()
 
         if return_dict:
@@ -179,15 +225,13 @@ class BaseModel(*_BASES):
 
     def set_counter(self, counter: int = 0):                        # base_model.py:27-31
         self.counter = counter
-        for module in self.model.modules():
-            if isinstance(module, BaseModule):
-                module.set_counter(counter)
+        for module in self._wrapped_modules():
+            module.set_counter(counter)
 
     def set_comm_manager(self, comm_manager: PatchParallelismCommManager):   # base_model.py:33-37
         self.comm_manager = comm_manager
-        for module in self.model.modules():
-            if isinstance(module, BaseModule):
-                module.set_comm_manager(comm_manager)
+        for module in self._wrapped_modules():
+            module.set_comm_manager(comm_manager)
 
     def setup_cuda_graph(self, static_outputs, cuda_graphs, graph_launches=None):   # base_model.py:39-41
         self.static_outputs = static_outputs

@@ -78,7 +78,9 @@ def row_plan(model: nn.Module, cfg: DistriConfig) -> list[int]:
 
 
 class DistriUNetPP(BaseModel):  # for Patch Parallelism
-    def __init__(self, model: nn.Module, distri_config: DistriConfig):
+    def __init__(self, model: nn.Module, distri_config: DistriConfig, controlnet: nn.Module | None = None):
+        """`controlnet` (optional): a ControlNetModel (or DistriControlNetPP) that forward() runs on this rank's strip before the
+        UNet, on the same epoch; its residuals go into the UNet without leaving the rank."""
         # the row plan (uneven strips when n does not divide the row units); one patch keeps the whole image, any height
         row_units = row_plan(model, distri_config) if distri_config.n_device_per_batch > 1 else None
         install_pp_wrappers(model, distri_config)
@@ -87,6 +89,13 @@ class DistriUNetPP(BaseModel):  # for Patch Parallelism
         for module in model.modules():
             if isinstance(module, BaseModule):
                 module.row_units = self.row_units
+        if controlnet is not None:
+            from .distri_controlnet_pp import DistriControlNetPP
+            if not isinstance(controlnet, DistriControlNetPP):
+                controlnet = DistriControlNetPP(controlnet, distri_config)
+            assert controlnet.row_units == self.row_units, (controlnet.row_units, self.row_units)
+            self.controlnet = controlnet
+            self._cn_scale = torch.ones(1, dtype=torch.float32, device=distri_config.device)
 
     def _strip(self, sample):
         h, w = sample.shape[2:]

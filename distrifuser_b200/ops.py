@@ -143,3 +143,26 @@ def linear_geglu(x: torch.Tensor, w_interleaved: torch.Tensor, b_interleaved: to
                                         x2.shape[0], N, K, x2.stride(0), w_interleaved.stride(0), 0, N // 2, 1, block, 0, 0, 0, 0, 0, 0, 0,
                                         torch.cuda.current_stream().cuda_stream), "df_linear_fwd")
     return out
+
+
+def controlnet_zero_convs(xs, convs, scale: torch.Tensor) -> list[torch.Tensor]:
+    """[scale * conv_i(xs[i]) for every 1x1 zero conv of a ControlNet call] in ONE launch (df_controlnet_zero_convs).  xs: fp16
+    NHWC activations; convs: the nn.Conv2d 1x1 modules; scale: a device fp32 tensor of one element, read by the kernel."""
+    import ctypes as C
+    n = len(xs)
+    assert len(convs) == n and scale.is_cuda and scale.dtype == torch.float32 and scale.numel() == 1
+    outs, xp, wp, bp, op, ms, ns, ks = [], [], [], [], [], [], [], []
+    for x, conv in zip(xs, convs):
+        assert x.is_cuda and x.dtype == torch.float16 and tuple(conv.kernel_size) == (1, 1)
+        x = x.contiguous(memory_format=torch.channels_last)
+        b, k, h, w = x.shape
+        out = torch.empty((b, conv.out_channels, h, w), dtype=x.dtype, device=x.device, memory_format=torch.channels_last)
+        outs.append(out)
+        xp.append(x.data_ptr()); wp.append(conv.weight.data_ptr()); op.append(out.data_ptr())
+        bp.append(conv.bias.data_ptr() if conv.bias is not None else None)
+        ms.append(b * h * w); ns.append(conv.out_channels); ks.append(k)
+    ptrs = lambda v: (C.c_void_p * n)(*v)
+    _lib.check(_lib.lib().df_controlnet_zero_convs(n, ptrs(xp), ptrs(wp), ptrs(bp), ptrs(op), (C.c_int64 * n)(*ms),
+                                                   (C.c_int32 * n)(*ns), (C.c_int32 * n)(*ks), scale.data_ptr(), 0,
+                                                   torch.cuda.current_stream().cuda_stream), "df_controlnet_zero_convs")
+    return outs

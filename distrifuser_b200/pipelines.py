@@ -12,10 +12,12 @@ from .models.naive_patch_sdxl import NaivePatchUNet
 from .utils import DistriConfig, PatchParallelismCommManager
 
 
-def _wrap(unet, distri_config: DistriConfig):
+def _wrap(unet, distri_config: DistriConfig, controlnet=None):
     if distri_config.parallelism == "patch":                         # pipelines.py:30-37
-        return DistriUNetPP(unet, distri_config)
+        return DistriUNetPP(unet, distri_config, controlnet=controlnet)
     if distri_config.parallelism == "naive_patch":
+        if controlnet is not None:
+            raise NotImplementedError("a ControlNet runs under patch parallelism only (parallelism='patch')")
         return NaivePatchUNet(unet, distri_config)
     raise ValueError(f"Unknown / unsupported parallelism: {distri_config.parallelism}")
 
@@ -34,6 +36,8 @@ class _DistriPipelineBase:
 
     @torch.no_grad()
     def __call__(self, *args, **kwargs):                             # pipelines.py:47-58
+        """With a ControlNet: image=[1, 3, height, width] (the conditioning image, shared by both CFG branches) and
+        controlnet_conditioning_scale=1.0, as in diffusers' ControlNet pipelines."""
         assert "height" not in kwargs, "height should not be in kwargs"
         assert "width" not in kwargs, "width should not be in kwargs"
         config = self.distri_config
@@ -55,6 +59,12 @@ class _DistriPipelineBase:
         assert cfg.height % 8 == 0 and cfg.width % 8 == 0
         static_inputs = self._static_inputs(**kwargs)
         unet = pipeline.unet
+        if getattr(unet, "controlnet", None) is not None:
+            # the conditioning image (both CFG branches share it) and the device scale the zero-conv kernel reads
+            B = static_inputs["sample"].shape[0]
+            static_inputs["controlnet_cond"] = torch.zeros((B, 3, cfg.height, cfg.width), dtype=static_inputs["sample"].dtype,
+                                                           device=cfg.device)
+            static_inputs["conditioning_scale"] = unet._cn_scale
         # cuDNN's default heuristics are not always the fastest 3x3 algorithm at these shapes; autotuning happens in the
         # un-captured passes below
         torch.backends.cudnn.benchmark = True
@@ -136,8 +146,9 @@ class DistriSDXLPipeline(_DistriPipelineBase):
 
     @staticmethod
     def from_synthetic(distri_config: DistriConfig, unet=None, unet_config: dict | None = None, seed: int = 0,
-                       scheduler=None, torch_dtype=torch.float16):
-        """Random-weight SDXL UNet (torch default init under manual_seed(seed), SURVEY 8d) + latent pipeline."""
+                       scheduler=None, torch_dtype=torch.float16, controlnet=None):
+        """Random-weight SDXL UNet (torch default init under manual_seed(seed), SURVEY 8d) + latent pipeline.
+        `controlnet`: a compat ControlNetModel run patch-parallel inside every UNet call (the pipeline then takes image=...)."""
         from .compat.pipeline import SyntheticLatentPipeline
         from .compat.unet_2d_condition import SDXL, UNet2DConditionModel
         if unet is None:
@@ -145,7 +156,9 @@ class DistriSDXLPipeline(_DistriPipelineBase):
             with torch.device(distri_config.device):
                 unet = UNet2DConditionModel(**(unet_config or SDXL))
         unet = unet.to(distri_config.device, torch_dtype).eval()
-        unet = _wrap(unet, distri_config)
+        if controlnet is not None:
+            controlnet = controlnet.to(distri_config.device, torch_dtype).eval()
+        unet = _wrap(unet, distri_config, controlnet)
         pipe = SyntheticLatentPipeline(unet, scheduler, sdxl=True, device=distri_config.device, dtype=torch_dtype)
         return DistriSDXLPipeline(pipe, distri_config)
 
@@ -194,7 +207,7 @@ class DistriSDPipeline(_DistriPipelineBase):
 
     @staticmethod
     def from_synthetic(distri_config: DistriConfig, unet=None, unet_config: dict | None = None, seed: int = 0,
-                       scheduler=None, torch_dtype=torch.float16):
+                       scheduler=None, torch_dtype=torch.float16, controlnet=None):
         from .compat.pipeline import SyntheticLatentPipeline
         from .compat.unet_2d_condition import SD15, UNet2DConditionModel
         if unet is None:
@@ -202,7 +215,9 @@ class DistriSDPipeline(_DistriPipelineBase):
             with torch.device(distri_config.device):
                 unet = UNet2DConditionModel(**(unet_config or SD15))
         unet = unet.to(distri_config.device, torch_dtype).eval()
-        unet = _wrap(unet, distri_config)
+        if controlnet is not None:
+            controlnet = controlnet.to(distri_config.device, torch_dtype).eval()
+        unet = _wrap(unet, distri_config, controlnet)
         pipe = SyntheticLatentPipeline(unet, scheduler, sdxl=False, device=distri_config.device, dtype=torch_dtype)
         return DistriSDPipeline(pipe, distri_config)
 

@@ -35,6 +35,7 @@ extern "C" {
 #define DF_MAX_WORLD 8
 #define DF_IPC_HANDLE_BYTES 64
 #define DF_TENSORMAP_BYTES 128
+#define DF_ZERO_CONV_MAX_PROBLEMS 13   /* zero convs of one ControlNet call: SDXL 10, SD1.x 13 */
 
 /* ---- errors / info ------------------------------------------------------------------------------ */
 const char* df_last_error(void);
@@ -229,6 +230,18 @@ int df_linear_fwd(df_comm_t comm, const void* a, const void* w, const void* bias
                   int64_t M, int N, int K, int64_t lda, int64_t ldw, int64_t ldr, int64_t ldo, int epilogue,
                   int geglu_block, int publish, int pub_col0, int idx, uint32_t peer_mask, uint64_t tensor_off,
                   uint64_t slot_bytes, int max_ctas, void* stream);
+
+/* ---- ControlNet zero convolutions: every 1x1 zero conv of one ControlNet call (SDXL 9 down + 1 mid, SD1.x 12 + 1) in ONE
+ *      persistent launch of the wgmma GEMM above:
+ *        out_i[M_i, N_i] = scale[0] * (x_i[M_i, K_i] . w_i[N_i, K_i]^T + bias_i[N_i])      i < nproblems <= DF_ZERO_CONV_MAX_PROBLEMS
+ *      x_i: the NHWC activation as a contiguous [b*h*w, C] fp16 matrix, w_i: the [N, K, 1, 1] weight, out_i contiguous.
+ *      The conv output is rounded to fp16 before the multiply, as torch computes `conv(x) * scale` (fp32 accumulate).
+ *      `scale` is a DEVICE fp32 read by the kernel, so a captured graph honours a new conditioning scale on every replay.
+ *      Each problem needs N % 8 == 0, K % 8 == 0 and 16-byte aligned x, w, bias (nullable) and out; the host checks them
+ *      before any launch.  The argument arrays are host arrays of nproblems entries; max_ctas: 0 = all SMs. ---------------- */
+int df_controlnet_zero_convs(int nproblems, const void* const* x_host, const void* const* w_host, const void* const* bias_host,
+                             void* const* out_host, const int64_t* m_host, const int32_t* n_host, const int32_t* k_host,
+                             const float* scale, int max_ctas, void* stream);
 
 #ifdef __cplusplus
 }
