@@ -13,7 +13,7 @@ import torch
 from torch import nn
 from torch.nn import functional as F
 
-from .unet_2d_condition import SDXL, TimestepEmbedding, UNet2DConditionModel, _Down, _Mid, sinusoid
+from .unet_2d_condition import SDXL, TimestepEmbedding, UNet2DConditionModel, _Down, _Mid, embed
 
 COND_CHANNELS = (16, 32, 96, 256)
 
@@ -107,19 +107,7 @@ class ControlNetModel(nn.Module):
                 added_cond_kwargs=None, return_dict=False):
         """-> (down_block_res_samples, mid_block_res_sample), each multiplied by conditioning_scale (a float, or a device
         tensor of one element that a captured graph re-reads on every replay)."""
-        c = self.config
-        t = timestep
-        if not torch.is_tensor(t):
-            t = torch.tensor([t], dtype=torch.float32, device=sample.device)
-        elif t.ndim == 0:
-            t = t[None]
-        t = t.to(sample.device).expand(sample.shape[0])
-        emb = self.time_embedding(sinusoid(t, c.block_out_channels[0]).to(sample.dtype))
-        if c.addition_embed_type == "text_time":
-            text, ids = added_cond_kwargs["text_embeds"], added_cond_kwargs["time_ids"]
-            tid = sinusoid(ids.flatten(), c.addition_time_embed_dim).reshape(text.shape[0], -1)
-            emb = emb + self.add_embedding(torch.cat([text, tid.to(text.dtype)], dim=-1).to(emb.dtype))
-        self._batched_temb(emb)
+        emb = embed(self, sample, timestep, added_cond_kwargs)
         x = self.conv_in(sample) + self.controlnet_cond_embedding(controlnet_cond)
         skips = [x]
         for blk in self.down_blocks:

@@ -343,6 +343,25 @@ def sinusoid(t: torch.Tensor, dim: int) -> torch.Tensor:
     return torch.cat([torch.cos(ang), torch.sin(ang)], dim=-1)
 
 
+def embed(model, sample, timestep, added_cond_kwargs):
+    """Time embedding of a UNet or ControlNet call plus SDXL's added (text_time) embedding -> emb [B, temb]; also hands every
+    ResnetBlock2D its projection of emb (model._batched_temb)."""
+    c = model.config
+    t = timestep
+    if not torch.is_tensor(t):
+        t = torch.tensor([t], dtype=torch.float32, device=sample.device)
+    elif t.ndim == 0:
+        t = t[None]
+    t = t.to(sample.device).expand(sample.shape[0])
+    emb = model.time_embedding(sinusoid(t, c.block_out_channels[0]).to(sample.dtype))
+    if c.addition_embed_type == "text_time":
+        text, ids = added_cond_kwargs["text_embeds"], added_cond_kwargs["time_ids"]
+        tid = sinusoid(ids.flatten(), c.addition_time_embed_dim).reshape(text.shape[0], -1)
+        emb = emb + model.add_embedding(torch.cat([text, tid.to(text.dtype)], dim=-1).to(emb.dtype))
+    model._batched_temb(emb)
+    return emb
+
+
 class UNet2DConditionModel(nn.Module):
     def __init__(self, **overrides):
         super().__init__()
@@ -426,19 +445,7 @@ class UNet2DConditionModel(nn.Module):
                 cross_attention_kwargs=None, added_cond_kwargs=None, down_block_additional_residuals=None,
                 mid_block_additional_residual=None, down_intrablock_additional_residuals=None,
                 encoder_attention_mask=None, return_dict=True):
-        c = self.config
-        t = timestep
-        if not torch.is_tensor(t):
-            t = torch.tensor([t], dtype=torch.float32, device=sample.device)
-        elif t.ndim == 0:
-            t = t[None]
-        t = t.to(sample.device).expand(sample.shape[0])
-        emb = self.time_embedding(sinusoid(t, c.block_out_channels[0]).to(sample.dtype))
-        if c.addition_embed_type == "text_time":
-            text, ids = added_cond_kwargs["text_embeds"], added_cond_kwargs["time_ids"]
-            tid = sinusoid(ids.flatten(), c.addition_time_embed_dim).reshape(text.shape[0], -1)
-            emb = emb + self.add_embedding(torch.cat([text, tid.to(text.dtype)], dim=-1).to(emb.dtype))
-        self._batched_temb(emb)
+        emb = embed(self, sample, timestep, added_cond_kwargs)
         x = self.conv_in(sample)
         skips = [x]
         for blk in self.down_blocks:

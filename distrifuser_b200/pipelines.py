@@ -31,6 +31,24 @@ class _DistriPipelineBase:
         self.static_inputs = None
         self.prepare()
 
+    @classmethod
+    def from_synthetic(cls, distri_config: DistriConfig, unet=None, unet_config: dict | None = None, seed: int = 0,
+                       scheduler=None, torch_dtype=torch.float16, controlnet=None):
+        """Random-weight SDXL / SD1.x UNet (torch default init under manual_seed(seed), SURVEY 8d) + latent pipeline.
+        `controlnet`: a compat ControlNetModel run patch-parallel inside every UNet call (the pipeline then takes image=...)."""
+        from .compat.pipeline import SyntheticLatentPipeline
+        from .compat.unet_2d_condition import SD15, SDXL, UNet2DConditionModel
+        if unet is None:
+            torch.manual_seed(seed)
+            with torch.device(distri_config.device):
+                unet = UNet2DConditionModel(**(unet_config or (SDXL if cls.sdxl else SD15)))
+        unet = unet.to(distri_config.device, torch_dtype).eval()
+        if controlnet is not None:
+            controlnet = controlnet.to(distri_config.device, torch_dtype).eval()
+        unet = _wrap(unet, distri_config, controlnet)
+        pipe = SyntheticLatentPipeline(unet, scheduler, sdxl=cls.sdxl, device=distri_config.device, dtype=torch_dtype)
+        return cls(pipe, distri_config)
+
     def set_progress_bar_config(self, **kwargs):                     # pipelines.py:44-45
         self.pipeline.set_progress_bar_config(**kwargs)
 
@@ -144,24 +162,6 @@ class DistriSDXLPipeline(_DistriPipelineBase):
         pipeline = StableDiffusionXLPipeline.from_pretrained(name, torch_dtype=torch_dtype, unet=unet, **kwargs).to(device)
         return DistriSDXLPipeline(pipeline, distri_config)
 
-    @staticmethod
-    def from_synthetic(distri_config: DistriConfig, unet=None, unet_config: dict | None = None, seed: int = 0,
-                       scheduler=None, torch_dtype=torch.float16, controlnet=None):
-        """Random-weight SDXL UNet (torch default init under manual_seed(seed), SURVEY 8d) + latent pipeline.
-        `controlnet`: a compat ControlNetModel run patch-parallel inside every UNet call (the pipeline then takes image=...)."""
-        from .compat.pipeline import SyntheticLatentPipeline
-        from .compat.unet_2d_condition import SDXL, UNet2DConditionModel
-        if unet is None:
-            torch.manual_seed(seed)
-            with torch.device(distri_config.device):
-                unet = UNet2DConditionModel(**(unet_config or SDXL))
-        unet = unet.to(distri_config.device, torch_dtype).eval()
-        if controlnet is not None:
-            controlnet = controlnet.to(distri_config.device, torch_dtype).eval()
-        unet = _wrap(unet, distri_config, controlnet)
-        pipe = SyntheticLatentPipeline(unet, scheduler, sdxl=True, device=distri_config.device, dtype=torch_dtype)
-        return DistriSDXLPipeline(pipe, distri_config)
-
     def _static_inputs(self, **kwargs):                              # pipelines.py:62-129
         cfg, pipeline = self.distri_config, self.pipeline
         device = cfg.device
@@ -204,22 +204,6 @@ class DistriSDPipeline(_DistriPipelineBase):
         unet = _wrap(unet, distri_config)
         pipeline = StableDiffusionPipeline.from_pretrained(name, torch_dtype=torch_dtype, unet=unet, **kwargs).to(device)
         return DistriSDPipeline(pipeline, distri_config)
-
-    @staticmethod
-    def from_synthetic(distri_config: DistriConfig, unet=None, unet_config: dict | None = None, seed: int = 0,
-                       scheduler=None, torch_dtype=torch.float16, controlnet=None):
-        from .compat.pipeline import SyntheticLatentPipeline
-        from .compat.unet_2d_condition import SD15, UNet2DConditionModel
-        if unet is None:
-            torch.manual_seed(seed)
-            with torch.device(distri_config.device):
-                unet = UNet2DConditionModel(**(unet_config or SD15))
-        unet = unet.to(distri_config.device, torch_dtype).eval()
-        if controlnet is not None:
-            controlnet = controlnet.to(distri_config.device, torch_dtype).eval()
-        unet = _wrap(unet, distri_config, controlnet)
-        pipe = SyntheticLatentPipeline(unet, scheduler, sdxl=False, device=distri_config.device, dtype=torch_dtype)
-        return DistriSDPipeline(pipe, distri_config)
 
     def _static_inputs(self, **kwargs):                              # pipelines.py:219-259
         cfg, pipeline = self.distri_config, self.pipeline

@@ -120,6 +120,24 @@ class TimestepEmbedding(nn.Module):
         return self.linear_2(self.act(self.linear_1(x)))
 
 
+def embed(model, sample, timestep, added_cond_kwargs):
+    """Time embedding of a UNet or ControlNet call, plus SDXL's added (text_time) embedding: emb [B, temb]."""
+    timesteps = timestep
+    if not torch.is_tensor(timesteps):
+        timesteps = torch.tensor([timesteps], dtype=torch.int64, device=sample.device)
+    elif timesteps.ndim == 0:
+        timesteps = timesteps[None].to(sample.device)
+    timesteps = timesteps.expand(sample.shape[0])
+    emb = model.time_embedding(model.time_proj(timesteps).to(sample.dtype))
+    if model.config.addition_embed_type == "text_time":
+        text_embeds = added_cond_kwargs["text_embeds"]
+        time_ids = added_cond_kwargs["time_ids"]
+        time_embeds = model.add_time_proj(time_ids.flatten()).reshape(text_embeds.shape[0], -1)
+        add = torch.cat([text_embeds, time_embeds], dim=-1).to(emb.dtype)
+        emb = emb + model.add_embedding(add)
+    return emb
+
+
 # --------------------------------------------------------------------------- transformer
 class Transformer2DModel(nn.Module):
     def __init__(self, heads, head_dim, in_channels, depth, cross_dim, groups, use_linear_projection):
@@ -325,25 +343,17 @@ class UNet2DConditionModel(ModelMixin, ConfigMixin):
                 attention_mask=None, cross_attention_kwargs=None, added_cond_kwargs=None,
                 down_block_additional_residuals=None, mid_block_additional_residual=None,
                 down_intrablock_additional_residuals=None, encoder_attention_mask=None, return_dict=True):
-        timesteps = timestep
-        if not torch.is_tensor(timesteps):
-            timesteps = torch.tensor([timesteps], dtype=torch.int64, device=sample.device)
-        elif timesteps.ndim == 0:
-            timesteps = timesteps[None].to(sample.device)
-        timesteps = timesteps.expand(sample.shape[0])
-        emb = self.time_embedding(self.time_proj(timesteps).to(sample.dtype))
-        if self.config.addition_embed_type == "text_time":
-            text_embeds = added_cond_kwargs["text_embeds"]
-            time_ids = added_cond_kwargs["time_ids"]
-            time_embeds = self.add_time_proj(time_ids.flatten()).reshape(text_embeds.shape[0], -1)
-            add = torch.cat([text_embeds, time_embeds], dim=-1).to(emb.dtype)
-            emb = emb + self.add_embedding(add)
+        emb = embed(self, sample, timestep, added_cond_kwargs)
         sample = self.conv_in(sample)
         res = (sample,)
         for blk in self.down_blocks:
             sample, out = blk(sample, emb, encoder_hidden_states=encoder_hidden_states)
             res += out
+        if down_block_additional_residuals is not None:      # ControlNet: skip i + residual i
+            res = tuple(r + d for r, d in zip(res, down_block_additional_residuals, strict=True))
         sample = self.mid_block(sample, emb, encoder_hidden_states=encoder_hidden_states)
+        if mid_block_additional_residual is not None:
+            sample = sample + mid_block_additional_residual
         for blk in self.up_blocks:
             n = len(blk.resnets)
             r, res = res[-n:], res[:-n]

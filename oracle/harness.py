@@ -4,7 +4,8 @@
 `impl="reference"` runs the UNMODIFIED reference modules imported from /root/reference through the
                    diffusers stub (only possible in the build container; used by oracle/make_golden.py).
 The UNet drivers serve every UNet case type: patch parallelism on equal (UNetCase) or uneven (RaggedCase) row strips, and
-naive patch (naive_patch.NaiveCase); the case's config_kwargs() choose the wrapper.
+naive patch (naive_patch.NaiveCase); the case's config_kwargs() choose the wrapper.  With `controlnet=` they run UNet +
+ControlNet (ControlledUNet) under the same patch-parallel wrapper, whose surgery wraps both models' layers alike.
 Both follow the reference's own bring-up order (pipelines.py:131-145): registration pass, create buffers,
 pre-run pass, then `set_counter(0)` and the denoising calls (pipelines.py:57).
 """
@@ -161,6 +162,48 @@ def _unet_config(case, rank):
     return cfg
 
 
+class ControlledUNet(nn.Module):
+    """Runs ControlNet then UNet with the UNet's call signature; the conditioning image `cond` (batch 1) is shared by both CFG
+    branches.  `down_blocks` is the UNet's, so that OracleUNetPP derives the row plan from it."""
+
+    def __init__(self, unet, controlnet, cond, scale=1.0):
+        super().__init__()
+        self.unet, self.controlnet, self.cond, self.scale = unet, controlnet, cond, scale
+
+    @property
+    def down_blocks(self):
+        return self.unet.down_blocks
+
+    @property
+    def config(self):
+        return self.unet.config
+
+    def forward(self, sample, timestep, encoder_hidden_states, added_cond_kwargs=None, return_dict=False):
+        cond = self.cond.expand(sample.shape[0], -1, -1, -1)
+        down, mid = self.controlnet(sample, timestep, encoder_hidden_states, cond, self.scale,
+                                    added_cond_kwargs=added_cond_kwargs)
+        return self.unet(sample, timestep, encoder_hidden_states, added_cond_kwargs=added_cond_kwargs,
+                         down_block_additional_residuals=down, mid_block_additional_residual=mid, return_dict=False)
+
+
+def _check_controlnet(case, impl, controlnet):
+    if controlnet is not None and impl == "reference":
+        raise ValueError("the reference has no ControlNet: a ControlNet case runs on impl='oracle' only")
+    if controlnet is not None and case.config_kwargs().get("parallelism") == "naive_patch":
+        raise NotImplementedError("a ControlNet runs under patch parallelism only (parallelism='patch')")
+
+
+def _unet(case, controlnet=None, scale=1.0):
+    """The seeded UNet of the case, or with `controlnet` the UNet + ControlNet module: "drawn" is the seeded ControlNet with
+    its zero-initialised layers drawn (non-zero residuals), "zero" the one as initialised."""
+    from oracle import workloads as W
+    unet = W.make_unet(case.family, case.weight_seed)
+    if controlnet is None:
+        return unet
+    cn = W.make_controlnet(case.family, case.weight_seed, zero=controlnet == "zero")
+    return ControlledUNet(unet, cn, W.cond_image(case), scale)
+
+
 def _oracle_unet(unet, cfg, bessel=True):
     from oracle import pp_modules as P
     if cfg.parallelism == "naive_patch":
@@ -169,13 +212,13 @@ def _oracle_unet(unet, cfg, bessel=True):
     return P.OracleUNetPP(unet, cfg, bessel=bessel)
 
 
-def _unet_worker(rank, case, impl, bessel, row_units, port, outdir):
+def _unet_worker(rank, case, impl, bessel, row_units, controlnet, scale, port, outdir):
     _paths(impl)
     from oracle import workloads as W
     _init(rank, case.world_size, port)
     cfg = _unet_config(case, rank)
     ucfg = W.unet_config(case.family)
-    unet = W.make_unet(case.family, case.weight_seed)
+    unet = _unet(case, controlnet, scale)
     first = W.unet_inputs(case, 0, ucfg)
     outs = []
     with torch.no_grad():
@@ -225,11 +268,13 @@ def run_ranks(worker, case, *args):
         return [torch.load(os.path.join(d, f"rank{r}.pt")) for r in range(case.world_size)]
 
 
-def run_unet(case, impl="oracle", bessel=True, row_units=None):
+def run_unet(case, impl="oracle", bessel=True, row_units=None, controlnet=None, scale=1.0):
     """-> outs[step] = eps prediction [B,4,H,W] (asserted identical on every rank).  The case picks the UNet wrapper: patch
     parallelism (UNetCase, RaggedCase) or naive patch (NaiveCase).  `bessel=False` drops the oracle GroupNorm's local-count
-    Bessel factor; `row_units`, when given, is asserted to be the oracle's row plan."""
-    per_rank = run_ranks(_unet_worker, case, impl, bessel, row_units)
+    Bessel factor; `row_units`, when given, is asserted to be the oracle's row plan.  `controlnet` ("drawn" or "zero", see
+    _unet) runs UNet + ControlNet at conditioning scale `scale` on the case's conditioning image (workloads.cond_image)."""
+    _check_controlnet(case, impl, controlnet)
+    per_rank = run_ranks(_unet_worker, case, impl, bessel, row_units, controlnet, scale)
     for r in range(1, case.world_size):
         for a, b in zip(per_rank[0], per_rank[r]):
             assert torch.equal(a, b), "final output must be identical on all ranks (distri_sdxl_unet_pp.py:166-168)"
@@ -253,14 +298,14 @@ class _OracleUNetAdapter:
         return (self.model(sample, t, encoder_hidden_states, added_cond_kwargs=added_cond_kwargs),)
 
 
-def _traj_worker(rank, case, num_steps, guidance, port, outdir):
+def _traj_worker(rank, case, num_steps, guidance, controlnet, port, outdir):
     _paths("oracle")
     from oracle import workloads as W
     from distrifuser_b200.compat.pipeline import SyntheticLatentPipeline      # the denoising loop itself is shared code:
     _init(rank, case.world_size, port)                                       # only the UNet path differs between the arms
     cfg = _unet_config(case, rank)
     ucfg = W.unet_config(case.family)
-    unet = W.make_unet(case.family, case.weight_seed)
+    unet = _unet(case, controlnet)
     model = _oracle_unet(unet, cfg)
     model.prepare(W.unet_inputs(case, 0, ucfg))
     pipe = SyntheticLatentPipeline(_OracleUNetAdapter(model, unet.config), sdxl=ucfg.get("addition_embed_type") == "text_time",
@@ -276,9 +321,11 @@ def _traj_worker(rank, case, num_steps, guidance, port, outdir):
         dist.destroy_process_group()
 
 
-def run_trajectory(case, num_steps=8, guidance=5.0):
-    """Final latents of a `num_steps` Euler trajectory with the ORACLE UNet path (fp32 CPU) -> [1,4,H,W]."""
-    outs = run_ranks(_traj_worker, case, num_steps, guidance)
+def run_trajectory(case, num_steps=8, guidance=5.0, controlnet=None):
+    """Final latents of a `num_steps` Euler trajectory with the ORACLE UNet path (fp32 CPU) -> [1,4,H,W].  `controlnet` as
+    in run_unet, at scale 1."""
+    _check_controlnet(case, "oracle", controlnet)
+    outs = run_ranks(_traj_worker, case, num_steps, guidance, controlnet)
     for o in outs[1:]:
         assert torch.equal(o, outs[0])
     return outs[0]

@@ -12,6 +12,7 @@ import dataclasses
 from types import SimpleNamespace
 
 import torch
+from torch.nn import functional as F
 
 MODES = ("corrected_async_gn", "stale_gn", "sync_gn", "separate_gn", "full_sync", "no_sync")
 
@@ -143,6 +144,30 @@ def make_unet(family: str, seed: int = 0, dtype=torch.float32):
     torch.manual_seed(seed)
     unet = UNet2DConditionModel(**unet_config(family))
     return unet.to(dtype).eval()
+
+
+def make_controlnet(family: str, seed: int = 0, zero: bool = False, dtype=torch.float32):
+    """Seeded ControlNet.  zero=False also draws the zero-initialised layers (the conditioning network's conv_out and the
+    1x1 zero convs), so that the residuals are not zero and the parity tests see them."""
+    from diffusers.models.controlnet import ControlNetModel
+    torch.manual_seed(seed + 101)
+    cn = ControlNetModel(**unet_config(family))
+    if not zero:
+        g = torch.Generator().manual_seed(seed + 202)
+        with torch.no_grad():
+            for conv in [cn.controlnet_cond_embedding.conv_out, *cn.controlnet_down_blocks, cn.controlnet_mid_block]:
+                fan_in = conv.weight[0].numel()
+                conv.weight.copy_(torch.randn(conv.weight.shape, generator=g) * (0.5 / fan_in ** 0.5))
+                conv.bias.copy_(torch.randn(conv.bias.shape, generator=g) * 0.05)
+    return cn.to(dtype).eval()
+
+
+def cond_image(case, dtype=torch.float32):
+    """Seeded conditioning image [1, 3, 8 * latent rows, 8 * latent cols] in [-1, 1] with some spatial structure."""
+    S, T = case.hw
+    g = torch.Generator().manual_seed(case.input_seed + 17)
+    img = torch.rand(1, 3, S, T, generator=g) * 2 - 1
+    return F.interpolate(img, scale_factor=8, mode="bilinear", align_corners=False).to(dtype)
 
 
 def unet_inputs(case, step: int, cfg_dict: dict, dtype=torch.float32):

@@ -1,13 +1,14 @@
 """ControlNet without a GPU: the compat model against the diffusers-0.24 restatement, the zero-weight premise, the oracle's
 patch-parallel UNet + ControlNet against one device, and the host-side checks of the patch-parallel wrapper."""
+from dataclasses import replace
 from types import SimpleNamespace
 
 import pytest
 import torch
 
-import controlnet_oracle as CO
 from helpers import psnr
 from oracle import workloads as W
+from oracle.harness import run_unet
 
 TINY = ("tiny_sdxl", "tiny_sd15")
 
@@ -24,7 +25,7 @@ def _compat_pair(family, zero=False):
     from distrifuser_b200.compat.controlnet import ControlNetModel
     from distrifuser_b200.compat.unet_2d_condition import UNet2DConditionModel
     ucfg = W.unet_config(family)
-    stub_unet, stub_cn = W.make_unet(family, 0), CO.make_controlnet(family, 0, zero=zero)
+    stub_unet, stub_cn = W.make_unet(family, 0), W.make_controlnet(family, 0, zero=zero)
     unet, cn = UNet2DConditionModel(**ucfg).eval(), ControlNetModel(**ucfg).eval()
     unet.load_state_dict(stub_unet.state_dict(), strict=True)
     cn.load_state_dict(stub_cn.state_dict(), strict=True)
@@ -34,7 +35,7 @@ def _compat_pair(family, zero=False):
 def _inputs(family, ucfg, lat=16):
     case = W.UNetCase("cn", family=family, latent=lat)
     inp = W.unet_inputs(case, 0, ucfg)
-    return inp, CO.cond_image(case).expand(case.batch, -1, -1, -1)
+    return inp, W.cond_image(case).expand(case.batch, -1, -1, -1)
 
 
 @pytest.mark.parametrize("family", TINY)
@@ -51,8 +52,9 @@ def test_compat_controlnet_matches_restatement(family):
         for a, b in zip([*d, m], [*d_ref, m_ref]):
             assert b.abs().max() > 1e-3                                   # the drawn zero convs give non-zero residuals
             torch.testing.assert_close(a, b, rtol=0, atol=1e-5)
-        want = CO.unet_forward(stub_unet, inp["sample"], inp["timestep"], inp["encoder_hidden_states"],
-                               inp["added_cond_kwargs"], d_ref, m_ref)
+        want = stub_unet(inp["sample"], inp["timestep"], inp["encoder_hidden_states"],
+                         added_cond_kwargs=inp["added_cond_kwargs"], down_block_additional_residuals=d_ref,
+                         mid_block_additional_residual=m_ref, return_dict=False)[0]
         got = unet(inp["sample"], inp["timestep"], inp["encoder_hidden_states"], added_cond_kwargs=inp["added_cond_kwargs"],
                    down_block_additional_residuals=d, mid_block_additional_residual=m, return_dict=False)[0]
     torch.testing.assert_close(got, want, rtol=0, atol=1e-5)
@@ -103,8 +105,8 @@ FULL_SYNC_CASES = (
 def test_oracle_full_sync_equals_one_device(case):
     """Every exchange synchronous: the patch-parallel UNet + ControlNet is the one-device forward (uneven strips: without the
     local-count Bessel factor, which differs between strip heights)."""
-    got = CO.run_oracle(case, bessel=False)
-    want = CO.run_one_device(case)
+    got = run_unet(case, bessel=False, controlnet="drawn")
+    want = run_unet(replace(case, world_size=1), controlnet="drawn")
     for a, b in zip(got, want):
         torch.testing.assert_close(a, b, rtol=0, atol=1e-5)
 
@@ -118,7 +120,7 @@ ASYNC_PSNR_DB = 18.0
 
 def test_oracle_corrected_async_gn_psnr():
     case = W.UNetCase("cn_sdxl_w2_async", world_size=2, split_batch=False, mode="corrected_async_gn", steps=4)
-    got, want = CO.run_oracle(case), CO.run_one_device(case)
+    got, want = run_unet(case, controlnet="drawn"), run_unet(replace(case, world_size=1), controlnet="drawn")
     ps = [psnr(a, b) for a, b in zip(got, want)]
     print("corrected_async_gn PSNR per step:", [f"{p:.1f}" for p in ps])
     assert min(ps) > ASYNC_PSNR_DB, ps

@@ -1,14 +1,15 @@
 """ControlNet on the H100: the one-launch zero-conv kernel against fp32 torch, and the patch-parallel UNet + ControlNet product
-against the fp32 oracle (tests/controlnet_oracle.py), eager and with CUDA graphs.  With fewer GPUs than ranks the ranks share
-cuda:0, as in mp_product.py."""
+(mp_product.py) against the fp32 oracle (oracle/harness.py), eager and with CUDA graphs.  With fewer GPUs than ranks the ranks
+share cuda:0, as in mp_product.py."""
 import dataclasses
 
 import pytest
 import torch
 
-import controlnet_oracle as CO
+import mp_product as MP
 from helpers import check_parity, psnr
 from oracle import workloads as W
+from oracle.harness import run_trajectory, run_unet
 
 pytestmark = pytest.mark.gpu
 
@@ -99,15 +100,15 @@ CASES = (
 @pytest.mark.parametrize("use_graph", [False, True], ids=["eager", "graph"])
 @pytest.mark.parametrize("case", CASES, ids=lambda c: c.name)
 def test_unet_controlnet_vs_oracle(case, use_graph):
-    want = CO.run_oracle(case)
-    got = CO.run_product_unet(case, use_graph=use_graph)
+    want = run_unet(case, controlnet="drawn")
+    got = MP.run_product_unet(case, use_graph=use_graph, controlnet="drawn")
     check_parity(case.name, got, want, ranks_identical=True)
 
 
 def test_zero_controlnet_output_bit_identical():
     """A zero-initialised ControlNet adds exact zeros: the product output equals the same pipeline without a ControlNet."""
     case = W.UNetCase("cn_sdxl_w2_zero", world_size=2, split_batch=False, steps=3)
-    for r, (without, with_cn) in enumerate(CO.run_zero_premise(case)):
+    for r, (without, with_cn) in enumerate(MP.run_zero_premise(case)):
         for t, (x, y) in enumerate(zip(without, with_cn)):
             assert torch.equal(x, y), f"rank {r} step {t}: max |diff| {(x - y).abs().max():.3e}"
 
@@ -116,18 +117,18 @@ def test_graph_replay_honours_new_scale():
     """One captured graph, a different conditioning scale per step: each step matches the oracle at that scale."""
     case = W.UNetCase("cn_sdxl_w1_scale", world_size=1, steps=3)
     scales = [1.0, 0.5, 0.0]
-    got = CO.run_product_unet(case, use_graph=True, scale=scales)
+    got = MP.run_product_unet(case, use_graph=True, controlnet="drawn", scale=scales)
     for t, s in enumerate(scales):
-        want = CO.run_oracle(dataclasses.replace(case, steps=t + 1), scale=s)[t]
+        want = run_unet(dataclasses.replace(case, steps=t + 1), controlnet="drawn", scale=s)[t]
         check_parity(f"{case.name} scale {s}", [[got[0][t]]], [want])
 
 
 def test_pipeline_trajectory_with_controlnet():
     case = W.UNetCase("cn_sdxl_w2_traj", world_size=2, split_batch=False, warmup_steps=2)
-    got = CO.run_product_trajectory(case)
+    got = MP.run_product_trajectory(case, controlnet="drawn")
     for r in range(1, len(got)):
         assert torch.equal(got[r], got[0]), f"rank {r} final latents differ from rank 0"
-    want = CO.run_oracle_trajectory(case)
+    want = run_trajectory(case, controlnet="drawn")
     p = psnr(got[0], want)
     assert p > 35, f"trajectory PSNR {p:.1f} dB"
 
@@ -136,8 +137,8 @@ def test_full_size_sdxl_unet_controlnet_step_vs_oracle():
     """The full SDXL UNet and a full-size ControlNet (random init, drawn zero convs), 512x512, one CFG step, world 1, against the
     fp32 oracle; the bar of test_full_size_sdxl_unet_step_vs_oracle."""
     case = dataclasses.replace(W.UNetCase("cn_sdxl_full_512", family="sdxl", world_size=1, latent=64), steps=1)
-    got = CO.run_product_unet(case)[0][0]
-    want = CO.run_one_device(case)[0]
+    got = MP.run_product_unet(case, controlnet="drawn")[0][0]
+    want = run_unet(case, controlnet="drawn")[0]
     assert got.shape == want.shape == (2, 4, 64, 64)
     err = (got - want).abs()
     std = want.std().item()

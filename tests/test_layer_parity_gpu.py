@@ -258,9 +258,9 @@ class LayerParity:
 
 
 def _product(wl):
-    from mp_product import _setup
-    pipe, ucfg = _setup(0, wl.case(), 0, False)
-    return pipe, ucfg
+    from mp_product import _pipeline
+    case = wl.case()
+    return _pipeline(case, False), W.unet_config(case.family)
 
 
 def _call(pipe, ucfg, wl):
