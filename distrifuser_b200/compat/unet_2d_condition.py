@@ -102,7 +102,8 @@ class FeedForward(nn.Module):
         self.net = nn.ModuleList([GEGLU(dim, 4 * dim), nn.Dropout(0.0), nn.Linear(4 * dim, dim)])
 
     def forward(self, x):
-        return self.net[2](self.net[0](x))
+        from .. import ops
+        return ops.project("ff2", self.net[0](x), self.net[2])
 
 
 class BasicTransformerBlock(nn.Module):
@@ -159,7 +160,8 @@ class Transformer2DModel(nn.Module):
         res = x
         x = self.norm(x)
         if self.use_linear_projection:
-            t = self.proj_in(self._tokens(x))
+            from .. import ops
+            t = ops.project("proj", self._tokens(x), self.proj_in)
         else:
             t = self._tokens(self.proj_in(x))
         if t.is_cuda and t.dtype == torch.float16:
@@ -171,7 +173,7 @@ class Transformer2DModel(nn.Module):
             for blk in self.transformer_blocks:
                 t = blk(t, encoder_hidden_states=encoder_hidden_states)
         if self.use_linear_projection:
-            x = self._image(self.proj_out(t), h, w)
+            x = self._image(ops.project("proj", t, self.proj_out), h, w)
         else:
             x = self.proj_out(self._image(t, h, w))
         return x + res

@@ -13,10 +13,13 @@
 //
 // Kernel: persistent CTAs, one per SM, each owning 128 x BN output tiles (BN = 256, or 160 where that fills the SMs better).
 // Per 64-wide K block the producer TMA-loads 128 rows of A and BN rows of W into a SWIZZLE_128B ring; two consumer warpgroups
-// each issue m64nBNk16 wgmmas for their 64 rows with the fp32 accumulators in registers, release the stage once the wgmma that
-// read it has retired, and run the epilogue straight from the accumulator fragment.  The producer keeps loading the next tile's
-// K blocks while the consumers are in the epilogue.
-//   warps 0-7  two consumer warpgroups (rows 0-63, 64-127 of the tile)      warp 8   TMA producer (one lane)
+// each issue m64nBNk16 wgmmas for their 64 rows with the fp32 accumulators in registers and release the stage once the wgmma
+// that read it has retired.  At the end of a tile the consumers add the bias, round to fp16 and stmatrix the tile into a
+// staging buffer, then start the next tile's mainloop at once.  The epilogue warps read the staged tile in 16-byte vectors and
+// finish it while the tensor cores run the next tile: GEGLU gate, residual add, coalesced 16-byte stores of the output and of
+// the published columns.
+//   warps 0-7  two consumer warpgroups (rows 0-63, 64-127 of the tile)
+//   warp 8     TMA producer (one lane)                 warps 9-11  epilogue
 #include <math.h>
 #include <string.h>
 
@@ -29,19 +32,35 @@ namespace {
 
 constexpr int BM = 128;            // rows of A per tile (64 per consumer warpgroup)
 constexpr int BK = 64;             // one 128-byte swizzled row of fp16
-constexpr int NTHREADS = 288;      // warps 0-7: two consumer warpgroups, warp 8: TMA producer
 constexpr int NCONSUMER_WARPS = 8;
+constexpr int NCONSUMERS = 32 * NCONSUMER_WARPS;
+constexpr int NTHREADS = NCONSUMERS + 128;   // GEMM: warps 0-7 consumers, warp 8 TMA producer, warps 9-11 epilogue
+constexpr int NEPILOGUE = 96;
+constexpr int NTHREADS_ZC = NCONSUMERS + 32; // zero convs: warps 0-7 consumers (own epilogue), warp 8 TMA producer
+// registers per thread after setmaxnreg: 256 x CONSUMER_REGS + 128 x WG2_REGS = 384 x 168, what the block launches with
+constexpr int CONSUMER_REGS = 208, WG2_REGS = 88;
 constexpr uint32_t A_BYTES = BM * BK * 2;
 
 // BN = output-tile columns (W rows): 256 for large N and the GEGLU epilogue, 160 where 256 would leave SMs idle.  Stages: as
-// many as fit next to each other in the 227 KiB a block may use.
-template <int BN> struct Stages { static constexpr int value = BN == 256 ? 4 : 5; };
+// many as fit in the 227 KiB a block may use next to the GEMM's staging buffer (LinearSmem).
+template <int BN> struct Stages { static constexpr int value = BN == 256 ? 3 : 5; };
 
 template <int BN>
 struct __align__(1024) SmemT {
   __half a[Stages<BN>::value][BM * BK];
   __half b[Stages<BN>::value][BN * BK];      // BN * 128 B per stage: a multiple of 1 KiB for BN in {160, 256}
   uint64_t full[Stages<BN>::value], empty[Stages<BN>::value];
+};
+
+// Staged fp16 tile: rows of BN + 8 halves.  The 16-byte pad moves row r by r 16-byte units (BN = 256) or 5r (BN = 160) modulo
+// the 8 units of a 128-byte bank line, so the 8 row addresses of one stmatrix phase hit 8 different units: no bank conflicts.
+template <int BN> __host__ __device__ constexpr int stage_pitch() { return BN + 8; }
+
+template <int BN>
+struct __align__(1024) LinearSmem {
+  SmemT<BN> ring;
+  __half stg[BM * stage_pitch<BN>()];
+  uint64_t stg_full, stg_empty;              // staged tile written by the consumers / read by the epilogue warps
 };
 
 enum { EPI_PLAIN = 0, EPI_GEGLU = 1 };
@@ -76,6 +95,18 @@ __device__ __forceinline__ float gelu_erf(float x) {      // same approximation 
 }
 
 __device__ __forceinline__ float2 ld_h2f(const __half* p) { return __half22float2(*reinterpret_cast<const __half2*>(p)); }
+
+// four 8 x 8 fp16 matrices from the accumulator fragment layout into shared memory; lane l gives the address of row l % 8 of
+// matrix l / 8
+__device__ __forceinline__ void stmatrix_x4(uint32_t addr, uint32_t r0, uint32_t r1, uint32_t r2, uint32_t r3) {
+  asm volatile("stmatrix.sync.aligned.m8n8.x4.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(r0), "r"(r1), "r"(r2), "r"(r3)
+               : "memory");
+}
+
+union H8 {                                  // one 16-byte vector of 8 fp16
+  uint4 u;
+  __half2 h[4];
+};
 
 template <int BN>
 __device__ __forceinline__ void wgmma_tile(float* acc, uint64_t a_desc, uint64_t b_desc, uint32_t accumulate) {
@@ -129,7 +160,8 @@ __global__ void __launch_bounds__(NTHREADS, 1)
 linear_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant__ CUtensorMap tm_w, LinearArgs p) {
   static_assert(BN % 32 == 0 && BN <= 256 && (BN * BK * 2) % 1024 == 0, "tile shape");
   constexpr int STAGES = Stages<BN>::value;
-  using Smem = SmemT<BN>;
+  constexpr int SP = stage_pitch<BN>();
+  using Smem = LinearSmem<BN>;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   Smem& sm = *reinterpret_cast<Smem*>(smem_raw);
   if ((smem_u32(smem_raw) & 1023u) != 0) __trap();
@@ -138,76 +170,121 @@ linear_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant__ 
   const int kblocks = p.K / BK;
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < STAGES; ++s) { mbar_init(&sm.full[s], 1); mbar_init(&sm.empty[s], NCONSUMER_WARPS); }
+    for (int s = 0; s < STAGES; ++s) { mbar_init(&sm.ring.full[s], 1); mbar_init(&sm.ring.empty[s], NCONSUMER_WARPS); }
+    mbar_init(&sm.stg_full, NCONSUMERS);
+    mbar_init(&sm.stg_empty, NEPILOGUE);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
 
-  if (warp == NCONSUMER_WARPS) {
-    // =============================================================== TMA producer
-    if (lane == 0) {
-      prefetch_tmap(&tm_a);
-      prefetch_tmap(&tm_w);
-      uint32_t stage = 0, phase = 0;
-      for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x)
-        load_tile<BN>(sm, &tm_a, &tm_w, tile % p.tiles_m, tile / p.tiles_m, kblocks, stage, phase);
-    }
-  } else {
-    // =============================================================== consumers (warps 0-7): main loop + epilogue
+  if (warp < NCONSUMER_WARPS) {
+    // =============================================================== consumers (warps 0-7): mainloop, bias, stage the tile
+    setmaxnreg_inc<CONSUMER_REGS>();
     const int wg = warp >> 2;
     const int c4 = lane & 3;
-    const int rloc = wg * 64 + (warp & 3) * 16 + (lane >> 2);   // tile row of accumulator rows A (rloc) and B (rloc + 8)
-    uint32_t pub_epoch = 0;
-    if (p.publish) pub_epoch = p.comm.clock[0];
-    uint32_t stage = 0, phase = 0;
+    // stmatrix row address of this lane: matrix lane / 8 of an x4 holds rows 8 * (lane / 8 % 2) + lane % 8 of the warp's 16
+    // rows, columns 8 * (lane / 16) + [0, 8) of the pair of 8-column blocks the x4 stores
+    const int mrow = wg * 64 + (warp & 3) * 16 + ((lane >> 3) & 1) * 8 + (lane & 7);
+    const uint32_t st_addr = smem_u32(sm.stg) + (uint32_t)(mrow * SP + (lane >> 4) * 8) * 2u;
+    uint32_t stage = 0, phase = 0, sphase = 0;
     float acc[BN / 2];
     for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
-      const int tm = tile % p.tiles_m, tn = tile / p.tiles_m;
-      mma_tile<BN>(sm, acc, wg, lane, kblocks, stage, phase);
+      const int tn = tile / p.tiles_m;
+      // the bias pairs of this thread's columns, loaded before the mainloop so that their latency hides behind it
+      __half2 bias2[BN / 8];
 #pragma unroll
-      for (int h = 0; h < 2; ++h) {                        // accumulator rows A / B of this thread
-        const int64_t grow = (int64_t)tm * BM + rloc + 8 * h;
-        if (grow >= p.M) continue;
+      for (int i = 0; i < BN / 8; ++i) {
+        const int col = tn * BN + 8 * i + 2 * c4;         // GEGLU: the interleaved bias has the tile's column order
+        bias2[i] = p.bias && col < p.N ? *reinterpret_cast<const __half2*>(p.bias + col) : __float2half2_rn(0.f);
+      }
+      mma_tile<BN>(sm.ring, acc, wg, lane, kblocks, stage, phase);
+      mbar_wait(&sm.stg_empty, sphase ^ 1u);             // the epilogue warps have read the previous tile
+#pragma unroll
+      for (int j = 0; j < BN / 16; ++j) {
+        uint32_t r[4];
+#pragma unroll
+        for (int q = 0; q < 2; ++q) {
+          const int i = 2 * j + q;
+          const float2 bb = __half22float2(bias2[i]);
+          // fp32 + bias rounded to fp16: torch's Linear output (GEGLU: diffusers rounds the projection before the gate)
+          r[2 * q] = pack_h2(acc[4 * i] + bb.x, acc[4 * i + 1] + bb.y);
+          r[2 * q + 1] = pack_h2(acc[4 * i + 2] + bb.x, acc[4 * i + 3] + bb.y);
+        }
+        stmatrix_x4(st_addr + j * 32, r[0], r[1], r[2], r[3]);
+      }
+      mbar_arrive(&sm.stg_full);
+      sphase ^= 1u;
+    }
+  } else {
+    setmaxnreg_dec<WG2_REGS>();
+    if (warp == NCONSUMER_WARPS) {
+      // ============================================================= TMA producer
+      if (lane == 0) {
+        prefetch_tmap(&tm_a);
+        prefetch_tmap(&tm_w);
+        uint32_t stage = 0, phase = 0;
+        for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x)
+          load_tile<BN>(sm.ring, &tm_a, &tm_w, tile % p.tiles_m, tile / p.tiles_m, kblocks, stage, phase);
+      }
+    } else {
+      // ============================================================= epilogue (warps 9-11): staged tile -> global memory
+      const int et = threadIdx.x - (NCONSUMERS + 32);
+      uint32_t pub_epoch = 0;
+      if (p.publish) pub_epoch = p.comm.clock[0];
+      uint32_t sphase = 0;
+      for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
+        const int tm = tile % p.tiles_m, tn = tile / p.tiles_m;
+        mbar_wait(&sm.stg_full, sphase);
         if (EPI == EPI_GEGLU) {
-          // accumulator columns [0, BN/2) = hidden, [BN/2, BN) = gate of output columns [tn*BN/2, (tn+1)*BN/2); N % BN == 0
-          __half* dst = p.out + grow * p.ldo + tn * (BN / 2);
+          // staged columns [0, BN/2) = hidden, [BN/2, BN) = gate of output columns [tn*BN/2, (tn+1)*BN/2); N % BN == 0
+          constexpr int CH = BN / 16;                     // 16-byte output vectors per row
+          for (int v = et; v < BM * CH; v += NEPILOGUE) {
+            const int r = v / CH, c = v % CH;
+            const int64_t grow = (int64_t)tm * BM + r;
+            if (grow >= p.M) continue;
+            H8 hv, gv, o;
+            hv.u = *reinterpret_cast<const uint4*>(sm.stg + r * SP + 8 * c);
+            gv.u = *reinterpret_cast<const uint4*>(sm.stg + r * SP + 8 * (c + CH));
 #pragma unroll
-          for (int i = 0; i < BN / 16; ++i) {
-            const int c = 8 * i + 2 * c4;
-            float2 bh = make_float2(0.f, 0.f), bg = make_float2(0.f, 0.f);
-            if (p.bias) { bh = ld_h2f(p.bias + tn * BN + c); bg = ld_h2f(p.bias + tn * BN + BN / 2 + c); }
-            const float* hv = acc + 4 * i + 2 * h;
-            const float* gv = acc + 4 * (i + BN / 16) + 2 * h;
-            // diffusers rounds the projection to fp16 before hidden * gelu(gate): reproduce that rounding
-            const float2 hf = __half22float2(__floats2half2_rn(hv[0] + bh.x, hv[1] + bh.y));
-            const float2 gf = __half22float2(__floats2half2_rn(gv[0] + bg.x, gv[1] + bg.y));
-            *reinterpret_cast<__half2*>(dst + c) = __floats2half2_rn(hf.x * gelu_erf(gf.x), hf.y * gelu_erf(gf.y));
+            for (int k = 0; k < 4; ++k) {
+              const float2 hf = __half22float2(hv.h[k]), gf = __half22float2(gv.h[k]);
+              o.h[k] = __floats2half2_rn(hf.x * gelu_erf(gf.x), hf.y * gelu_erf(gf.y));
+            }
+            *reinterpret_cast<uint4*>(p.out + grow * p.ldo + tn * (BN / 2) + 8 * c) = o.u;
           }
         } else {
-          const int col0 = tn * BN;
-          __half* dst = p.out + grow * p.ldo + col0;
-          const __half* res = p.residual ? p.residual + grow * p.ldr + col0 : nullptr;
+          constexpr int CH = BN / 8;
+          // unrolled, with the residual read through the read-only path, so that the residual loads of several vectors are
+          // in flight at once
+#pragma unroll 4
+          for (int v = et; v < BM * CH; v += NEPILOGUE) {
+            const int r = v / CH, c = v % CH;
+            const int64_t grow = (int64_t)tm * BM + r;
+            const int col = tn * BN + 8 * c;
+            if (grow >= p.M || col >= p.N) continue;     // N % 8 == 0: a vector is entirely inside or outside
+            H8 o;
+            o.u = *reinterpret_cast<const uint4*>(sm.stg + r * SP + 8 * c);
+            if (p.residual) {                             // torch: fp16 linear output, then fp16 add
+              H8 rv;
+              rv.u = __ldg(reinterpret_cast<const uint4*>(p.residual + grow * p.ldr + col));
 #pragma unroll
-          for (int i = 0; i < BN / 8; ++i) {
-            const int c = 8 * i + 2 * c4;
-            const int col = col0 + c;
-            if (col >= p.N) continue;                      // N % 8 == 0: a column pair is entirely inside or outside
-            float2 f = make_float2(acc[4 * i + 2 * h], acc[4 * i + 2 * h + 1]);
-            if (p.bias) { const float2 bb = ld_h2f(p.bias + col); f.x += bb.x; f.y += bb.y; }
-            __half2 o = __floats2half2_rn(f.x, f.y);
-            if (res) o = __hadd2(o, *reinterpret_cast<const __half2*>(res + c));   // torch: fp16 linear output, then fp16 add
-            *reinterpret_cast<__half2*>(dst + c) = o;
-            if (p.publish && col >= p.pub_col0) {          // k|v columns: also into every peer's slot of the publish epoch
+              for (int k = 0; k < 4; ++k) o.h[k] = __hadd2(o.h[k], rv.h[k]);
+            }
+            *reinterpret_cast<uint4*>(p.out + grow * p.ldo + col) = o.u;
+            if (p.publish && col >= p.pub_col0) {         // k|v columns: also into every peer's slot of the publish epoch
               const uint64_t off = slot_offset(p.comm, pub_epoch, p.tensor_off, p.slot_bytes, p.comm.rank) +
                                    ((uint64_t)grow * p.pub_cols + (col - p.pub_col0)) * 2;
               for (int q = 0; q < p.comm.world; ++q)
-                if (p.peer_mask >> q & 1) *reinterpret_cast<__half2*>((char*)p.comm.base[q] + off) = o;
+                if (p.peer_mask >> q & 1) *reinterpret_cast<uint4*>((char*)p.comm.base[q] + off) = o.u;
             }
           }
         }
+        mbar_arrive(&sm.stg_empty);
+        sphase ^= 1u;
       }
     }
   }
+  // every thread fences its own peer stores before the CTA's ticket is taken
   if (p.publish) signal_when_last(p.comm, &p.comm.tickets[p.idx], gridDim.x, p.idx, p.peer_mask, p.comm.clock[0]);
 }
 
@@ -231,10 +308,10 @@ template <int EPI, int BN>
 int launch_linear(const CUtensorMap& ta, const CUtensorMap& tw, const LinearArgs& args, int ctas, cudaStream_t st) {
   static bool attr_set = false;
   if (!attr_set) {
-    DF_CHECK_CUDA(cudaFuncSetAttribute(linear_kernel<EPI, BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(SmemT<BN>)));
+    DF_CHECK_CUDA(cudaFuncSetAttribute(linear_kernel<EPI, BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(LinearSmem<BN>)));
     attr_set = true;
   }
-  linear_kernel<EPI, BN><<<ctas, NTHREADS, sizeof(SmemT<BN>), st>>>(ta, tw, args);
+  linear_kernel<EPI, BN><<<ctas, NTHREADS, sizeof(LinearSmem<BN>), st>>>(ta, tw, args);
   DF_CHECK_LAUNCH();
   return 0;
 }
@@ -302,6 +379,7 @@ extern "C" int df_linear_fwd(df_comm_t comm, const void* a, const void* w, const
   args.comm = comm;
   if (args.publish) {
     DF_REQUIRE(pub_col0 >= 0 && pub_col0 < N && pub_col0 % 8 == 0, "df_linear_fwd: bad pub_col0");
+    DF_REQUIRE(tensor_off % 16 == 0 && slot_bytes % 16 == 0, "df_linear_fwd: slots must be 16-byte aligned");
     args.pub_col0 = pub_col0; args.pub_cols = N - pub_col0; args.idx = idx; args.peer_mask = peer_mask;
     args.tensor_off = tensor_off; args.slot_bytes = slot_bytes;
     DF_REQUIRE((uint64_t)M * args.pub_cols * 2 <= slot_bytes, "df_linear_fwd: published columns larger than the slot");
@@ -351,7 +429,7 @@ __device__ __forceinline__ int zc_problem(const ZeroConvArgs& z, int tile) {
   return q;
 }
 
-__global__ void __launch_bounds__(NTHREADS, 1) zero_conv_kernel(const __grid_constant__ ZeroConvArgs z) {
+__global__ void __launch_bounds__(NTHREADS_ZC, 1) zero_conv_kernel(const __grid_constant__ ZeroConvArgs z) {
   constexpr int BN = ZC_BN;
   constexpr int STAGES = Stages<BN>::value;
   using Smem = SmemT<BN>;
@@ -451,7 +529,7 @@ extern "C" int df_controlnet_zero_convs(int nproblems, const void* const* x_host
     DF_CHECK_CUDA(cudaFuncSetAttribute(zero_conv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(SmemT<ZC_BN>)));
     attr_set = true;
   }
-  zero_conv_kernel<<<ctas, NTHREADS, sizeof(SmemT<ZC_BN>), (cudaStream_t)stream>>>(z);
+  zero_conv_kernel<<<ctas, NTHREADS_ZC, sizeof(SmemT<ZC_BN>), (cudaStream_t)stream>>>(z);
   DF_CHECK_LAUNCH();
   return 0;
 }

@@ -1,6 +1,7 @@
 """DistriSelfAttentionPP / DistriCrossAttentionPP -- drop-ins for distrifuser/modules/pp/attn.py:12-195.
 
-q / fused kv / out projections stay library GEMMs (cuBLAS through F.linear); everything between them --
+q / fused q|k|v / out projections are cuBLAS GEMMs unless DF_LINEAR puts them on the hand-written one (ops.linear /
+ops.project); everything between them --
 the reference's torch.cat of the per-rank K/V (attn.py:131-138), split / view / transpose (:142-149) and
 F.scaled_dot_product_attention (:153) -- is one wgmma kernel (df_attn_fwd) that TMA-loads the K/V tiles
 straight from the n per-rank segments: this rank's fresh projection and the peers' 1-step-stale arena slots."""
@@ -85,11 +86,10 @@ class DistriAttentionPP(BaseModule):
         return out
 
     def _project_out(self, hidden_states, residual, weight=None):
+        from ... import ops
         attn = self.module
-        if weight is not None:                                           # zero-padded head columns (see _qkv_weight)
-            hidden_states = F.linear(hidden_states, weight, attn.to_out[0].bias)
-        else:
-            hidden_states = attn.to_out[0](hidden_states)                # attn.py:93-96 / 158-161
+        # attn.py:93-96 / 158-161; weight: to_out with zero columns for the padded head dims (see _qkv_weight)
+        hidden_states = ops.project("out", hidden_states, attn.to_out[0], weight)
         hidden_states = attn.to_out[1](hidden_states)
         if attn.residual_connection:
             hidden_states = hidden_states + residual
@@ -108,7 +108,8 @@ class DistriCrossAttentionPP(DistriAttentionPP):
         assert encoder_hidden_states is not None                         # attn.py:55
         self._require_cuda_half(hidden_states, "DistriCrossAttentionPP")
         attn = self.module
-        q = attn.to_q(hidden_states)
+        from ... import ops
+        q = ops.project("qkv", hidden_states, attn.to_q)
         if self.counter == 0 or self.kv_cache is None:                   # attn.py:56,73-77: text K/V once per image
             kv = self.to_kv(encoder_hidden_states)
             if self.kv_cache is not None and self.kv_cache.shape == kv.shape:

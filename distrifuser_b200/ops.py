@@ -68,8 +68,8 @@ def conv2d_bias_residual(x: torch.Tensor, conv: torch.nn.Conv2d, padding, residu
 # ---------------------------------------------------------------------------------------------------- wgmma GEMM (csrc/linear.cu)
 
 # which Linear layers run on the hand-written GEMM: comma list out of {geglu, qkv, out, ff2, proj}; "all" / "none".
-# Default: the GEGLU projection, whose fused epilogue saves the [M, 8C] intermediate; tools/bench_linear.py compares the rest
-# with cuBLAS at the model's shapes.
+# Default: the GEGLU projection, whose fused epilogue saves the [M, 8C] intermediate.  The plain kinds are slower than cuBLAS at
+# the model's step shapes on H100 (tools/bench_linear.py, DESIGN §7), so they stay off by default.
 _FUSED_LINEAR = set(_os.environ.get("DF_LINEAR", "geglu").replace("all", "geglu,qkv,out,ff2,proj").split(","))
 
 
@@ -129,6 +129,22 @@ def linear(x: torch.Tensor, weight: torch.Tensor, bias: torch.Tensor | None = No
                                         int(publish is not None), pub_col0, idx, mask, off, sb, 0,
                                         torch.cuda.current_stream().cuda_stream), "df_linear_fwd")
     return out
+
+
+def project(kind: str, x: torch.Tensor, lin: torch.nn.Linear, weight: torch.Tensor | None = None) -> torch.Tensor:
+    """lin(x) for a transformer-block Linear of `kind` ("qkv", "out", "ff2", "proj"): on the hand-written GEMM when DF_LINEAR
+    selects the kind, else lin itself (cuBLAS).  `weight` replaces lin.weight (zero-padded to_out of narrow heads).  A Linear
+    with a LoRA layer attached keeps its own forward."""
+    w = lin.weight if weight is None else weight
+    K = x.shape[-1]
+    if (use_fused_linear(kind) and x.is_cuda and x.dtype == torch.float16 and w.dtype == torch.float16 and
+            x.stride(-1) == 1 and w.stride(-1) == 1 and getattr(lin, "lora_layer", None) is None and
+            linear_supported(x.numel() // K, w.shape[0], K)):
+        return linear(x, w, lin.bias)
+    if weight is None:
+        return lin(x)
+    import torch.nn.functional as F
+    return F.linear(x, weight, lin.bias)
 
 
 def linear_geglu(x: torch.Tensor, w_interleaved: torch.Tensor, b_interleaved: torch.Tensor | None, block: int = GEGLU_BLOCK) -> torch.Tensor:
