@@ -20,7 +20,7 @@ EXPORTS = (
     "df_symm_free", "df_step_begin", "df_slot_publish", "df_slot_wait", "df_groupnorm_scratch_bytes",
     "df_groupnorm_fwd", "df_groupnorm_halo_fwd", "df_groupnorm_fwd_weighted", "df_groupnorm_halo_fwd_weighted", "df_halo_push",
     "df_halo_assemble", "df_attn_make_kvmaps", "df_attn_workspace_bytes", "df_attn_fwd", "df_attn_make_kvmaps_ragged",
-    "df_attn_workspace_bytes_ragged", "df_attn_fwd_ragged",
+    "df_attn_workspace_bytes_ragged", "df_attn_fwd_ragged", "df_attn_wide_make_kvmaps", "df_attn_wide_fwd",
     "df_output_gather", "df_output_gather_2d", "df_geglu", "df_add_layernorm", "df_bias_residual_add", "df_linear_supported", "df_linear_geglu_block", "df_linear_fwd",
     "df_controlnet_zero_convs",
 )
@@ -70,6 +70,9 @@ def lib():
         L.df_attn_workspace_bytes_ragged.restype = C.c_size_t
         L.df_attn_fwd_ragged.argtypes = [DfComm, vp, vp, vp, vp, i32, i32, i32p, i32, i32, i64, i64, i64, i32, i32, i32p, i32,
                                          i32, f32, vp, C.c_size_t, vp]
+        L.df_attn_wide_make_kvmaps.argtypes = [DfComm, u64, u64, i32, i32p, i32, vp, vp]
+        L.df_attn_wide_fwd.argtypes = [DfComm, vp, vp, vp, vp, i32, i32, i32p, i32, i64, i64, i64, i32, i32, i32p, i32, i32, f32,
+                                       vp]
         L.df_halo_push.argtypes = [DfComm, vp, i32, i32, i32, i32, i32, u64, u64, i32, i32, vp]
         L.df_halo_assemble.argtypes = [DfComm, vp, vp, i32, i32, i32, i32, i32, u64, u64, i32, i32, i32, vp]
         L.df_attn_make_kvmaps.argtypes = [DfComm, u64, u64, i32, i32, i32, i32, vp, vp]
@@ -96,7 +99,7 @@ def lib():
 
 # kernels launched per C-ABI call (bench.py reports the count of OUR launches inside the timed region)
 KERNELS_PER_CALL = {"df_groupnorm_fwd": 1, "df_groupnorm_halo_fwd": 1, "df_attn_fwd": 1, "df_groupnorm_fwd_weighted": 1,
-                    "df_groupnorm_halo_fwd_weighted": 1, "df_attn_fwd_ragged": 1, "df_halo_push": 1, "df_halo_assemble": 1,
+                    "df_groupnorm_halo_fwd_weighted": 1, "df_attn_fwd_ragged": 1, "df_attn_wide_fwd": 1, "df_halo_push": 1, "df_halo_assemble": 1,
                     "df_slot_publish": 1, "df_slot_wait": 1, "df_step_begin": 1, "df_output_gather": 2, "df_output_gather_2d": 2, "df_geglu": 1, "df_add_layernorm": 1, "df_bias_residual_add": 1,
                     "df_linear_fwd": 1, "df_controlnet_zero_convs": 1}
 LAUNCHES = {"total": 0}

@@ -2,7 +2,7 @@
 
 It reproduces the part of the diffusers denoising loop the reference's hot path lives in (SURVEY 3.2): CFG batch
 duplication, scheduler.scale_model_input, one UNet call per step, guidance combine, scheduler.step.  Prompt
-encoding and the VAE are replaced by seeded synthetic embeddings / latent output (no weights exist here)."""
+encoding is replaced by seeded synthetic embeddings; with a VAE (compat.vae) output_type="pt" decodes the latents."""
 import hashlib
 from types import SimpleNamespace
 
@@ -12,8 +12,9 @@ from .schedulers import DDIMScheduler, EulerDiscreteScheduler
 
 
 class SyntheticLatentPipeline:
-    def __init__(self, unet, scheduler=None, sdxl: bool = True, device="cuda", dtype=torch.float16):
+    def __init__(self, unet, scheduler=None, sdxl: bool = True, device="cuda", dtype=torch.float16, vae=None):
         self.unet = unet
+        self.vae = vae
         self.scheduler = scheduler or (EulerDiscreteScheduler() if sdxl else DDIMScheduler())
         self.sdxl = sdxl
         self.device = torch.device(device)
@@ -55,7 +56,10 @@ class SyntheticLatentPipeline:
     def __call__(self, prompt="", height=1024, width=1024, num_inference_steps=50, guidance_scale=5.0, generator=None,
                  latents=None, output_type="latent", prompt_embeds=None, pooled_prompt_embeds=None, image=None,
                  controlnet_conditioning_scale=1.0, **kwargs):
-        """image: the ControlNet conditioning image [1, 3, height, width] when the UNet has a ControlNet attached."""
+        """image: the ControlNet conditioning image [1, 3, height, width] when the UNet has a ControlNet attached.
+        output_type: "pt" returns the VAE's image in [0, 1], [1, 3, height, width] (needs a VAE); anything else the final latents."""
+        if output_type == "pt" and self.vae is None:
+            raise ValueError("output_type='pt' needs a VAE: build the pipeline with vae=AutoencoderKL(...)")
         dev = self.device
         cfg_on = guidance_scale > 1.0
         if prompt_embeds is None:
@@ -94,4 +98,8 @@ class SyntheticLatentPipeline:
                 e_u, e_c = eps.float().chunk(2)
                 eps = e_u + guidance_scale * (e_c - e_u)
             lat = self.scheduler.step(eps, t, lat)[0]
+        if output_type == "pt":                                      # diffusers: decode, then the image processor's denormalise
+            image = self.vae.decode((lat / self.vae.config.scaling_factor).to(self.dtype), return_dict=False,
+                                    generator=generator)[0]
+            return SimpleNamespace(images=(image / 2 + 0.5).clamp(0, 1))
         return SimpleNamespace(images=lat)

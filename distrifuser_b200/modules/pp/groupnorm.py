@@ -19,6 +19,9 @@ class DistriGroupNorm(BaseModule):
         assert isinstance(module, nn.GroupNorm)
         super().__init__(module, distri_config)
         self.fuse_silu = False          # set by the block-level fusion in DistriUNetPP
+        # True: the variance is always the biased one of nn.GroupNorm (the exact statistics of the whole image when the
+        # exchange is synchronous); False keeps the reference's local-count Bessel factor in the exchanging modes
+        self.biased_var = False
         self._scratch = None
 
     def _plan(self):
@@ -55,6 +58,8 @@ class DistriGroupNorm(BaseModule):
             # exchange needs a slot in every mode that synchronises (sync_gn / full_sync / warm-up steps)
             self.idx = self.comm_manager.register_tensor([2, b, G, 1, 1, 1], torch.float32, layer_type="gn")
         mode, bessel, neg_fb = self._plan()
+        if self.biased_var:
+            bessel = 0
         x = x.contiguous(memory_format=torch.channels_last)
         halo = pad_for.halo_plan(x) if pad_for is not None else None
         if halo is None:

@@ -8,8 +8,18 @@ and a latent-space pipeline stand-in (compat/pipeline.py): that is what bench.py
 import torch
 
 from .models.distri_sdxl_unet_pp import DistriUNetPP
+from .models.distri_vae_pp import DistriAutoencoderKLPP
 from .models.naive_patch_sdxl import NaivePatchUNet
 from .utils import DistriConfig, PatchParallelismCommManager
+
+
+def _distribute_vae(pipeline, distri_config: DistriConfig, distributed_vae: bool):
+    """distributed_vae=True: the pipeline's own VAE decodes patch-parallel on every rank (DistriAutoencoderKLPP)."""
+    if distributed_vae:
+        if getattr(pipeline, "vae", None) is None:
+            raise ValueError("distributed_vae=True, but the pipeline has no VAE")
+        pipeline.vae = DistriAutoencoderKLPP(pipeline.vae, distri_config)
+    return pipeline
 
 
 def _wrap(unet, distri_config: DistriConfig, controlnet=None):
@@ -33,9 +43,11 @@ class _DistriPipelineBase:
 
     @classmethod
     def from_synthetic(cls, distri_config: DistriConfig, unet=None, unet_config: dict | None = None, seed: int = 0,
-                       scheduler=None, torch_dtype=torch.float16, controlnet=None):
+                       scheduler=None, torch_dtype=torch.float16, controlnet=None, vae=None):
         """Random-weight SDXL / SD1.x UNet (torch default init under manual_seed(seed), SURVEY 8d) + latent pipeline.
-        `controlnet`: a compat ControlNetModel run patch-parallel inside every UNet call (the pipeline then takes image=...)."""
+        `controlnet`: a compat ControlNetModel run patch-parallel inside every UNet call (the pipeline then takes image=...).
+        `vae`: an AutoencoderKL (compat.vae) whose decoder runs patch-parallel on every rank (DistriAutoencoderKLPP); the
+        pipeline then also returns images with output_type="pt"."""
         from .compat.pipeline import SyntheticLatentPipeline
         from .compat.unet_2d_condition import SD15, SDXL, UNet2DConditionModel
         if unet is None:
@@ -46,7 +58,9 @@ class _DistriPipelineBase:
         if controlnet is not None:
             controlnet = controlnet.to(distri_config.device, torch_dtype).eval()
         unet = _wrap(unet, distri_config, controlnet)
-        pipe = SyntheticLatentPipeline(unet, scheduler, sdxl=cls.sdxl, device=distri_config.device, dtype=torch_dtype)
+        if vae is not None:
+            vae = DistriAutoencoderKLPP(vae.to(distri_config.device, torch_dtype).eval(), distri_config)
+        pipe = SyntheticLatentPipeline(unet, scheduler, sdxl=cls.sdxl, device=distri_config.device, dtype=torch_dtype, vae=vae)
         return cls(pipe, distri_config)
 
     def set_progress_bar_config(self, **kwargs):                     # pipelines.py:44-45
@@ -157,9 +171,11 @@ class DistriSDXLPipeline(_DistriPipelineBase):
         device = distri_config.device
         name = kwargs.pop("pretrained_model_name_or_path", "stabilityai/stable-diffusion-xl-base-1.0")
         torch_dtype = kwargs.pop("torch_dtype", torch.float16)
+        distributed_vae = kwargs.pop("distributed_vae", False)      # True: the VAE decode runs split over every rank
         unet = UNet2DConditionModel.from_pretrained(name, torch_dtype=torch_dtype, subfolder="unet").to(device)
         unet = _wrap(unet, distri_config)
         pipeline = StableDiffusionXLPipeline.from_pretrained(name, torch_dtype=torch_dtype, unet=unet, **kwargs).to(device)
+        pipeline = _distribute_vae(pipeline, distri_config, distributed_vae)
         return DistriSDXLPipeline(pipeline, distri_config)
 
     def _static_inputs(self, **kwargs):                              # pipelines.py:62-129
@@ -200,9 +216,11 @@ class DistriSDPipeline(_DistriPipelineBase):
         device = distri_config.device
         name = kwargs.pop("pretrained_model_name_or_path", "CompVis/stable-diffusion-v1-4")
         torch_dtype = kwargs.pop("torch_dtype", torch.float16)
+        distributed_vae = kwargs.pop("distributed_vae", False)      # True: the VAE decode runs split over every rank
         unet = UNet2DConditionModel.from_pretrained(name, torch_dtype=torch_dtype, subfolder="unet").to(device)
         unet = _wrap(unet, distri_config)
         pipeline = StableDiffusionPipeline.from_pretrained(name, torch_dtype=torch_dtype, unet=unet, **kwargs).to(device)
+        pipeline = _distribute_vae(pipeline, distri_config, distributed_vae)
         return DistriSDPipeline(pipeline, distri_config)
 
     def _static_inputs(self, **kwargs):                              # pipelines.py:219-259

@@ -180,6 +180,19 @@ int df_attn_fwd_ragged(df_comm_t comm, const void* q, const void* kv_own, void* 
                        int64_t o_pitch, int nseg, int own_seg, const int32_t* seg_rank_host, int idx, int wait_flags, float scale,
                        void* workspace, size_t workspace_bytes, void* stream);
 
+/* ---- attention for ONE head of width 512 (the VAE decoder's mid-block attention, diffusers Attention with heads = 1,
+ *      dim_head = 512), which df_attn_fwd (d <= 192) does not cover.  Same segment layout as df_attn_fwd_ragged with heads = 1:
+ *      q:[b,lq,512] fp16 (pitch q_pitch elements), out same shape (pitch o_pitch); K/V in `nseg` segments of seg_len_host[s]
+ *      rows, each [b, len_s, 1024] (K at column 0, V at 512); segment own_seg is kv_own (pitch kv_pitch), every other segment s
+ *      is read from slot(read%NB, idx, src=seg_rank[s]) through the tensor maps of df_attn_wide_make_kvmaps (seg_len_host[s] =
+ *      rows held by communicator member s).  wait_flags != 0: the kernel acquires the peers' flags itself.  fp32 softmax and
+ *      accumulators; scale 0 = 1/sqrt(512).  d must be 512. */
+int df_attn_wide_make_kvmaps(df_comm_t comm, uint64_t tensor_off, uint64_t slot_bytes, int b, const int32_t* seg_len_host, int d,
+                             void* maps_out /* device, DF_NBANKS*world*DF_TENSORMAP_BYTES */, void* stream);
+int df_attn_wide_fwd(df_comm_t comm, const void* q, const void* kv_own, void* out, const void* kvmaps, int b, int lq,
+                     const int32_t* seg_len_host, int d, int64_t q_pitch, int64_t kv_pitch, int64_t o_pitch, int nseg, int own_seg,
+                     const int32_t* seg_rank_host, int idx, int wait_flags, float scale, void* stream);
+
 /* ---- final epsilon gather: replaces the blocking world all_gather + cat(dim=2) at the end of
  *      DistriUNetPP.forward (distrifuser/models/distri_sdxl_unet_pp.py:162-169,186-193).
  *      strip: this rank's [bs,C,hs,W] NCHW fp16 output; it is written into slot(pub%NB, idx, 0) of every
