@@ -14,6 +14,7 @@ MAX_WORLD = 8
 IPC_HANDLE_BYTES = 64
 TENSORMAP_BYTES = 128
 ZERO_CONV_MAX_PROBLEMS = 13
+F16, F32 = 0, 1                  # element types of the *_dtype calls (DF_F16 / DF_F32)
 
 EXPORTS = (
     "df_last_error", "df_version", "df_device_sm_count", "df_symm_alloc", "df_symm_open", "df_symm_close",
@@ -22,7 +23,8 @@ EXPORTS = (
     "df_halo_assemble", "df_attn_make_kvmaps", "df_attn_workspace_bytes", "df_attn_fwd", "df_attn_make_kvmaps_ragged",
     "df_attn_workspace_bytes_ragged", "df_attn_fwd_ragged", "df_attn_wide_make_kvmaps", "df_attn_wide_fwd",
     "df_output_gather", "df_output_gather_2d", "df_geglu", "df_add_layernorm", "df_bias_residual_add", "df_linear_supported", "df_linear_geglu_block", "df_linear_fwd",
-    "df_controlnet_zero_convs",
+    "df_controlnet_zero_convs", "df_groupnorm_scratch_bytes_dtype", "df_groupnorm_fwd_dtype", "df_groupnorm_halo_fwd_dtype",
+    "df_halo_push_dtype", "df_halo_assemble_dtype", "df_output_gather_2d_dtype",
 )
 
 
@@ -65,6 +67,10 @@ def lib():
                                                 i32, u64, u64, u32, i32p, vp, vp]
         L.df_groupnorm_halo_fwd_weighted.argtypes = [DfComm, vp, vp, i64, vp, vp, vp, i32, i32, i32, i32, i32, f32, i32, i32, i32,
                                                      i32, i32, u64, u64, u32, i32p, vp, i32, u64, u64, i32, i32, i32, i32, vp]
+        L.df_groupnorm_scratch_bytes_dtype.argtypes = [i32, i32, i32, i32, i32, i32]
+        L.df_groupnorm_scratch_bytes_dtype.restype = C.c_size_t
+        L.df_groupnorm_fwd_dtype.argtypes = L.df_groupnorm_fwd_weighted.argtypes[:-1] + [i32, vp]
+        L.df_groupnorm_halo_fwd_dtype.argtypes = L.df_groupnorm_halo_fwd_weighted.argtypes[:-1] + [i32, vp]
         L.df_attn_make_kvmaps_ragged.argtypes = [DfComm, u64, u64, i32, i32p, i32, i32, vp, vp]
         L.df_attn_workspace_bytes_ragged.argtypes = [i32, i32, i32p, i32, i32, i32]
         L.df_attn_workspace_bytes_ragged.restype = C.c_size_t
@@ -75,6 +81,8 @@ def lib():
                                        vp]
         L.df_halo_push.argtypes = [DfComm, vp, i32, i32, i32, i32, i32, u64, u64, i32, i32, vp]
         L.df_halo_assemble.argtypes = [DfComm, vp, vp, i32, i32, i32, i32, i32, u64, u64, i32, i32, i32, vp]
+        L.df_halo_push_dtype.argtypes = L.df_halo_push.argtypes[:-1] + [i32, vp]
+        L.df_halo_assemble_dtype.argtypes = L.df_halo_assemble.argtypes[:-1] + [i32, vp]
         L.df_attn_make_kvmaps.argtypes = [DfComm, u64, u64, i32, i32, i32, i32, vp, vp]
         L.df_attn_workspace_bytes.argtypes = [i32, i32, i32, i32, i32, i32]
         L.df_attn_workspace_bytes.restype = C.c_size_t
@@ -91,6 +99,7 @@ def lib():
                                                C.POINTER(i64), C.POINTER(C.c_int32), C.POINTER(C.c_int32), vp, i32, vp]
         L.df_output_gather.argtypes = [DfComm, vp, vp, i32, i32, i32, i32, i32, i32, i32, i32, i32, u64, vp]
         L.df_output_gather_2d.argtypes = [DfComm, vp, vp, i32, i32, i32, i32, i32, i32, i32, i32, i32, i32, i32, u64, vp]
+        L.df_output_gather_2d_dtype.argtypes = L.df_output_gather_2d.argtypes[:-1] + [i32, vp]
         for name in EXPORTS:
             getattr(L, name)  # AttributeError if the header and the library disagree
         _lib = L
@@ -101,7 +110,8 @@ def lib():
 KERNELS_PER_CALL = {"df_groupnorm_fwd": 1, "df_groupnorm_halo_fwd": 1, "df_attn_fwd": 1, "df_groupnorm_fwd_weighted": 1,
                     "df_groupnorm_halo_fwd_weighted": 1, "df_attn_fwd_ragged": 1, "df_attn_wide_fwd": 1, "df_halo_push": 1, "df_halo_assemble": 1,
                     "df_slot_publish": 1, "df_slot_wait": 1, "df_step_begin": 1, "df_output_gather": 2, "df_output_gather_2d": 2, "df_geglu": 1, "df_add_layernorm": 1, "df_bias_residual_add": 1,
-                    "df_linear_fwd": 1, "df_controlnet_zero_convs": 1}
+                    "df_linear_fwd": 1, "df_controlnet_zero_convs": 1, "df_groupnorm_fwd_dtype": 1, "df_groupnorm_halo_fwd_dtype": 1,
+                    "df_halo_push_dtype": 1, "df_halo_assemble_dtype": 1, "df_output_gather_2d_dtype": 2}
 LAUNCHES = {"total": 0}
 PROFILE = None   # bench.py sets this to a list; kernels then bracket their launch with CUDA events on the launching stream
 
@@ -117,6 +127,15 @@ def int32_array(values) -> C.Array:
     values = list(values)
     assert len(values) <= MAX_WORLD
     return (C.c_int32 * MAX_WORLD)(*values)
+
+
+def dtype_code(dtype) -> int:
+    """The element type of a *_dtype call for a torch dtype: fp16 or fp32 (anything else is refused)."""
+    import torch
+    codes = {torch.float16: F16, torch.float32: F32}
+    if dtype not in codes:
+        raise RuntimeError(f"distrifuser_b200 kernels take fp16 or fp32 tensors, not {dtype}")
+    return codes[dtype]
 
 
 def null_comm() -> DfComm:

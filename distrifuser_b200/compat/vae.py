@@ -149,6 +149,9 @@ class Decoder(nn.Module):
 
     def forward(self, z):
         x = self.mid_block(self.conv_in(z))
+        # diffusers' Decoder.forward: the up blocks run in their own dtype (fp32 under StableDiffusionXLPipeline.upcast_vae(),
+        # which leaves conv_in and the mid block in fp16)
+        x = x.to(next(iter(self.up_blocks.parameters())).dtype)
         for blk in self.up_blocks:
             x = blk(x)
         if self.fused_norm_act and hasattr(self.conv_out, "halo_plan") and self.conv_out.halo_plan(x) is not None:

@@ -168,13 +168,14 @@ extern "C" int df_slot_wait(df_comm_t comm, int idx, uint32_t src_mask, void* st
 
 // ------------------------------------------------------------------------------------ final epsilon gather
 // Each (batch, channel) plane of the strip is `rows` runs of `vpr` vectors; run r lands at row row0 + r, column col0 of the
-// image plane.  A full-width strip is one run of hs*W elements (rows = 1), so it vectorises whenever hs*W does.
-template <typename V>
+// image plane.  A full-width strip is one run of hs*W elements (rows = 1), so it vectorises whenever hs*W does.  V: the access
+// (a 16-byte vector or one element), ES: the element size in bytes.
+template <typename V, int ES>
 __global__ void __launch_bounds__(256) out_scatter_kernel(df_comm_t c, const V* __restrict__ strip, int C, int H, int W,
                                                           int bs, int rows, int vpr, int batch0, int row0, int col0, int idx,
                                                           uint64_t tensor_off, uint32_t world_mask) {
   const uint32_t epoch = c.clock[2];
-  constexpr int E = sizeof(V) / 2;
+  constexpr int E = sizeof(V) / ES;
   const int plane = rows * vpr;                    // vectors per (batch, channel) plane of the strip
   const int64_t total = (int64_t)bs * C * plane;
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
@@ -186,7 +187,7 @@ __global__ void __launch_bounds__(256) out_scatter_kernel(df_comm_t c, const V* 
     V v = strip[i];
     int64_t dst_el = (((int64_t)(batch0 + bb) * C + ch) * H + row0 + r) * W + col0 + (int64_t)q * E;
     for (int p = 0; p < c.world; ++p) {
-      V* d = (V*)(slot_ptr(c, p, epoch, tensor_off, 0, 0) + dst_el * 2);
+      V* d = (V*)(slot_ptr(c, p, epoch, tensor_off, 0, 0) + dst_el * ES);
       *d = v;
     }
   }
@@ -203,49 +204,72 @@ __global__ void __launch_bounds__(256) out_collect_kernel(df_comm_t c, V* __rest
     out[i] = src[i];
 }
 
-// Scatter of a strip made of bs*C planes of `rows` runs of `run` elements, then the collect of the whole image.  `vec_shape`:
-// the runs and their destinations are whole 8-element vectors.
+// Scatter of a strip made of bs*C planes of `rows` runs of `run` elements of T, then the collect of the whole image.
+// `vec_shape`: the runs and their destinations are whole 16-byte vectors.
+template <typename T>
 static int output_gather(df_comm_t comm, const void* strip, void* out, int B, int C, int H, int W, int bs, int rows, int run,
                          int batch0, int row0, int col0, bool vec_shape, int idx, uint64_t tensor_off, void* stream) {
+  constexpr int ES = sizeof(T), E = 16 / ES;
   uint32_t mask = comm.world >= 32 ? 0xffffffffu : ((1u << comm.world) - 1u);
   int64_t strip_el = (int64_t)bs * C * rows * run, total_el = (int64_t)B * C * H * W;
   bool vec = vec_shape && ((uintptr_t)strip % 16) == 0 && ((uintptr_t)out % 16) == 0 && tensor_off % 16 == 0;
   cudaStream_t st = (cudaStream_t)stream;
   if (vec) {
-    int g1 = (int)((strip_el / 8 + 255) / 256); g1 = g1 < 1 ? 1 : (g1 > 64 ? 64 : g1);
-    out_scatter_kernel<int4><<<g1, 256, 0, st>>>(comm, (const int4*)strip, C, H, W, bs, rows, run / 8, batch0, row0, col0, idx,
-                                                 tensor_off, mask);
+    int g1 = (int)((strip_el / E + 255) / 256); g1 = g1 < 1 ? 1 : (g1 > 64 ? 64 : g1);
+    out_scatter_kernel<int4, ES><<<g1, 256, 0, st>>>(comm, (const int4*)strip, C, H, W, bs, rows, run / E, batch0, row0, col0,
+                                                     idx, tensor_off, mask);
     DF_CHECK_LAUNCH();
-    int g2 = (int)((total_el / 8 + 255) / 256); g2 = g2 < 1 ? 1 : (g2 > 64 ? 64 : g2);
-    out_collect_kernel<int4><<<g2, 256, 0, st>>>(comm, (int4*)out, total_el / 8, idx, tensor_off);
+    int g2 = (int)((total_el / E + 255) / 256); g2 = g2 < 1 ? 1 : (g2 > 64 ? 64 : g2);
+    out_collect_kernel<int4><<<g2, 256, 0, st>>>(comm, (int4*)out, total_el / E, idx, tensor_off);
     DF_CHECK_LAUNCH();
   } else {
     int g1 = (int)((strip_el + 255) / 256); g1 = g1 < 1 ? 1 : (g1 > 64 ? 64 : g1);
-    out_scatter_kernel<__half><<<g1, 256, 0, st>>>(comm, (const __half*)strip, C, H, W, bs, rows, run, batch0, row0, col0, idx,
-                                                   tensor_off, mask);
+    out_scatter_kernel<T, ES><<<g1, 256, 0, st>>>(comm, (const T*)strip, C, H, W, bs, rows, run, batch0, row0, col0, idx,
+                                                  tensor_off, mask);
     DF_CHECK_LAUNCH();
     int g2 = (int)((total_el + 255) / 256); g2 = g2 < 1 ? 1 : (g2 > 64 ? 64 : g2);
-    out_collect_kernel<__half><<<g2, 256, 0, st>>>(comm, (__half*)out, total_el, idx, tensor_off);
+    out_collect_kernel<T><<<g2, 256, 0, st>>>(comm, (T*)out, total_el, idx, tensor_off);
     DF_CHECK_LAUNCH();
   }
   return 0;
 }
 
+// A full-width strip is one run per plane; it takes the 16-byte path only when every plane's run starts on a vector (the image
+// plane H*W and the strip's offset row0*W are whole vectors) and is whole vectors long.
+static bool full_width_vec(int H, int W, int hs, int row0, int E) {
+  return (int64_t)hs * W % E == 0 && (int64_t)row0 * W % E == 0 && (int64_t)H * W % E == 0;
+}
+
 extern "C" int df_output_gather(df_comm_t comm, const void* strip, void* out, int B, int C, int H, int W, int bs, int hs,
                                 int batch0, int row0, int idx, uint64_t tensor_off, void* stream) {
   DF_REQUIRE(batch0 + bs <= B && row0 + hs <= H, "df_output_gather: strip outside the image");
-  return output_gather(comm, strip, out, B, C, H, W, bs, 1, hs * W, batch0, row0, 0, (hs * W) % 8 == 0, idx, tensor_off,
-                       stream);
+  return output_gather<__half>(comm, strip, out, B, C, H, W, bs, 1, hs * W, batch0, row0, 0, full_width_vec(H, W, hs, row0, 8), idx,
+                               tensor_off, stream);
 }
 
-extern "C" int df_output_gather_2d(df_comm_t comm, const void* strip, void* out, int B, int C, int H, int W, int bs, int hs,
-                                   int ws, int batch0, int row0, int col0, int idx, uint64_t tensor_off, void* stream) {
+template <typename T>
+static int output_gather_2d(df_comm_t comm, const void* strip, void* out, int B, int C, int H, int W, int bs, int hs, int ws,
+                            int batch0, int row0, int col0, int idx, uint64_t tensor_off, void* stream) {
+  constexpr int E = 16 / sizeof(T);
   DF_REQUIRE(bs > 0 && hs > 0 && ws > 0 && batch0 >= 0 && row0 >= 0 && col0 >= 0,
              "df_output_gather_2d: bad strip (bs=%d hs=%d ws=%d at %d,%d,%d)", bs, hs, ws, batch0, row0, col0);
   DF_REQUIRE(batch0 + bs <= B && row0 + hs <= H && col0 + ws <= W, "df_output_gather_2d: strip outside the image");
   if (ws == W)                                      // full-width strip: one contiguous run per plane, as df_output_gather
-    return output_gather(comm, strip, out, B, C, H, W, bs, 1, hs * W, batch0, row0, 0, (hs * W) % 8 == 0, idx, tensor_off,
-                         stream);
-  return output_gather(comm, strip, out, B, C, H, W, bs, hs, ws, batch0, row0, col0, ws % 8 == 0 && col0 % 8 == 0 && W % 8 == 0,
-                       idx, tensor_off, stream);
+    return output_gather<T>(comm, strip, out, B, C, H, W, bs, 1, hs * W, batch0, row0, 0, full_width_vec(H, W, hs, row0, E), idx,
+                            tensor_off, stream);
+  return output_gather<T>(comm, strip, out, B, C, H, W, bs, hs, ws, batch0, row0, col0, ws % E == 0 && col0 % E == 0 && W % E == 0,
+                          idx, tensor_off, stream);
+}
+
+extern "C" int df_output_gather_2d_dtype(df_comm_t comm, const void* strip, void* out, int B, int C, int H, int W, int bs, int hs,
+                                         int ws, int batch0, int row0, int col0, int idx, uint64_t tensor_off, int dtype,
+                                         void* stream) {
+  DF_REQUIRE(dtype == DF_F16 || dtype == DF_F32, "df_output_gather_2d: unknown element type %d", dtype);
+  return (dtype == DF_F32 ? output_gather_2d<float> : output_gather_2d<__half>)(comm, strip, out, B, C, H, W, bs, hs, ws, batch0,
+                                                                                row0, col0, idx, tensor_off, stream);
+}
+
+extern "C" int df_output_gather_2d(df_comm_t comm, const void* strip, void* out, int B, int C, int H, int W, int bs, int hs,
+                                   int ws, int batch0, int row0, int col0, int idx, uint64_t tensor_off, void* stream) {
+  return df_output_gather_2d_dtype(comm, strip, out, B, C, H, W, bs, hs, ws, batch0, row0, col0, idx, tensor_off, DF_F16, stream);
 }

@@ -1,10 +1,10 @@
-// distrifuser_b200 -- 3x3-conv halo exchange (NHWC fp16, one halo row).
+// distrifuser_b200 -- 3x3-conv halo exchange (NHWC fp16 or fp32, one halo row).
 // Replaces the boundary torch.stack + all_gather over ALL ranks + cat/F.pad of DistriConv2dPP.forward
 // (distrifuser/modules/pp/conv2d.py:72-93): rows travel to the two patch neighbours only, written straight
 // into their arena slots with 16-byte peer stores, and the padded conv input is assembled by one coalesced
 // vectorised kernel.
 //
-// Slot layout of tensor idx, source s:  [2][b][w*C] halves  -- part 0 = s's first row, part 1 = s's last row
+// Slot layout of tensor idx, source s:  [2][b][w*C] elements  -- part 0 = s's first row, part 1 = s's last row
 // (the reference's buffer_list[s][0] / [s][1], conv2d.py:61-65,90).
 #include "common.cuh"
 
@@ -57,9 +57,13 @@ __global__ void __launch_bounds__(256) halo_assemble_kernel(df_comm_t c, const c
 
 }  // namespace
 
-extern "C" int df_halo_push(df_comm_t comm, const void* x, int b, int h, int w, int C, int idx, uint64_t tensor_off,
-                            uint64_t slot_bytes, int up_rank, int down_rank, void* stream) {
-  uint64_t row_bytes = (uint64_t)w * C * 2;
+// the kernels copy bytes: the element type only sets the row size
+static uint64_t halo_row_bytes(int w, int C, int dtype) { return (uint64_t)w * C * (dtype == DF_F32 ? 4 : 2); }
+
+extern "C" int df_halo_push_dtype(df_comm_t comm, const void* x, int b, int h, int w, int C, int idx, uint64_t tensor_off,
+                                  uint64_t slot_bytes, int up_rank, int down_rank, int dtype, void* stream) {
+  DF_REQUIRE(dtype == DF_F16 || dtype == DF_F32, "df_halo_push: unknown element type %d", dtype);
+  uint64_t row_bytes = halo_row_bytes(w, C, dtype);
   DF_REQUIRE(row_bytes % 16 == 0 && ((uintptr_t)x % 16) == 0, "df_halo_push: rows must be 16-byte multiples");
   DF_REQUIRE(slot_bytes >= 2ull * b * row_bytes, "df_halo_push: slot too small");
   if (up_rank < 0 && down_rank < 0) return 0;
@@ -72,10 +76,11 @@ extern "C" int df_halo_push(df_comm_t comm, const void* x, int b, int h, int w, 
   return 0;
 }
 
-extern "C" int df_halo_assemble(df_comm_t comm, const void* x, void* xp, int b, int h, int w, int C, int idx,
-                                uint64_t tensor_off, uint64_t slot_bytes, int up_rank, int down_rank, int wait_flags,
-                                void* stream) {
-  uint64_t row_bytes = (uint64_t)w * C * 2;
+extern "C" int df_halo_assemble_dtype(df_comm_t comm, const void* x, void* xp, int b, int h, int w, int C, int idx,
+                                      uint64_t tensor_off, uint64_t slot_bytes, int up_rank, int down_rank, int wait_flags,
+                                      int dtype, void* stream) {
+  DF_REQUIRE(dtype == DF_F16 || dtype == DF_F32, "df_halo_assemble: unknown element type %d", dtype);
+  uint64_t row_bytes = halo_row_bytes(w, C, dtype);
   DF_REQUIRE(row_bytes % 16 == 0 && ((uintptr_t)x % 16) == 0 && ((uintptr_t)xp % 16) == 0,
              "df_halo_assemble: rows must be 16-byte multiples");
   uint64_t total = (uint64_t)b * (h + 2) * (row_bytes / 16);
@@ -85,4 +90,16 @@ extern "C" int df_halo_assemble(df_comm_t comm, const void* x, void* xp, int b, 
                                                               tensor_off, slot_bytes, up_rank, down_rank, wait_flags);
   DF_CHECK_LAUNCH();
   return 0;
+}
+
+extern "C" int df_halo_push(df_comm_t comm, const void* x, int b, int h, int w, int C, int idx, uint64_t tensor_off,
+                            uint64_t slot_bytes, int up_rank, int down_rank, void* stream) {
+  return df_halo_push_dtype(comm, x, b, h, w, C, idx, tensor_off, slot_bytes, up_rank, down_rank, DF_F16, stream);
+}
+
+extern "C" int df_halo_assemble(df_comm_t comm, const void* x, void* xp, int b, int h, int w, int C, int idx,
+                                uint64_t tensor_off, uint64_t slot_bytes, int up_rank, int down_rank, int wait_flags,
+                                void* stream) {
+  return df_halo_assemble_dtype(comm, x, xp, b, h, w, C, idx, tensor_off, slot_bytes, up_rank, down_rank, wait_flags, DF_F16,
+                                stream);
 }

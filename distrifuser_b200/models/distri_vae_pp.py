@@ -10,7 +10,11 @@ decode up to fp16 rounding:
   * mid-block attention: every rank's K/V segment through the arena, df_attn_wide_fwd (DistriVAEAttentionPP);
   * the [B, 3, 8h, 8w] image: df_output_gather_2d, which is also the per-call world barrier the arena's banks rely on
     (BANK-REUSE INVARIANT, utils.py).
-The decoder has its own PatchParallelismCommManager (arena, flags, epoch clock), so the UNet's arena is untouched."""
+The decoder has its own PatchParallelismCommManager (arena, flags, epoch clock), so the UNet's arena is untouched.
+
+upcast=True decodes a VAE that overflows fp16 (force_upcast, e.g. the stock SDXL VAE) with the precision split of diffusers'
+StableDiffusionXLPipeline.upcast_vae(): post_quant_conv, conv_in and the mid block (with its attention) in fp16, the up blocks,
+conv_norm_out and conv_out in fp32.  The GroupNorm, halo and gather kernels then run their fp32 instantiations there."""
 import copy
 
 import torch
@@ -30,9 +34,14 @@ def _is_vae_attention(m: nn.Module) -> bool:
     return all(hasattr(m, a) for a in ("to_q", "to_k", "to_v", "to_out", "group_norm"))
 
 
-def install_vae_wrappers(decoder: nn.Module, distri_config: DistriConfig) -> None:
+# the decoder's parts that diffusers' upcast_vae() leaves in fp32 (everything after the mid block)
+UPCAST_PARTS = ("up_blocks", "conv_norm_out", "conv_out")
+
+
+def install_vae_wrappers(decoder: nn.Module, distri_config: DistriConfig, upcast: bool = False) -> None:
     """Module surgery of the decoder in place: 3x3 convs, GroupNorms (biased variance) and the mid-block attention become the
-    sm_90a wrappers, GroupNorm -> SiLU pairs fuse, and the decoder goes channels_last."""
+    sm_90a wrappers, GroupNorm -> SiLU pairs fuse, and the decoder goes channels_last.  upcast: the wrappers of UPCAST_PARTS
+    take fp32 tensors."""
     for _, module in list(decoder.named_modules()):
         if isinstance(module, BaseModule) or _is_vae_attention(module):
             continue
@@ -54,7 +63,21 @@ def install_vae_wrappers(decoder: nn.Module, distri_config: DistriConfig) -> Non
                 sub = getattr(module, nm, None)
                 if isinstance(sub, DistriGroupNorm):
                     sub.fuse_silu = True
+    if upcast:
+        for part in UPCAST_PARTS:
+            for module in getattr(decoder, part).modules():
+                if isinstance(module, BaseModule):
+                    module.allow_fp32 = True
     decoder.to(memory_format=torch.channels_last)
+
+
+def apply_upcast_split(vae: nn.Module) -> None:
+    """diffusers' upcast_vae() precision split, whatever the VAE's dtype: the decoder's UPCAST_PARTS in fp32, post_quant_conv,
+    conv_in and the mid block in fp16."""
+    for m in (vae.post_quant_conv, vae.decoder.conv_in, vae.decoder.mid_block):
+        m.to(torch.float16)
+    for part in UPCAST_PARTS:
+        getattr(vae.decoder, part).to(torch.float32)
 
 
 def vae_row_plan(latent_rows: int, world: int) -> list[int]:
@@ -66,15 +89,21 @@ def vae_row_plan(latent_rows: int, world: int) -> list[int]:
 
 
 class DistriAutoencoderKLPP(nn.Module):
-    """Wraps an AutoencoderKL (compat.vae or diffusers) for fp16 decoding on every rank; `decode(z, return_dict=True)` and
-    `config` as diffusers' AutoencoderKL, so a diffusers pipeline's own `self.vae.decode(...)` runs it."""
+    """Wraps an AutoencoderKL (compat.vae or diffusers) for decoding on every rank; `decode(z, return_dict=True)` and
+    `config` as diffusers' AutoencoderKL, so a diffusers pipeline's own `self.vae.decode(...)` runs it.
 
-    def __init__(self, vae: nn.Module, distri_config: DistriConfig):
+    upcast=False: the decode runs in fp16 and returns fp16; a VAE whose config sets force_upcast is refused.
+    upcast=True: any VAE, with diffusers' precision split (module docstring); decode() takes fp16 latents and returns an fp32
+    image.  `config` then reports force_upcast=False (a copy: the VAE's own config is left alone) and `dtype` is fp16, so a
+    diffusers SDXL pipeline passes its fp16 latents straight to decode() instead of calling upcast_vae() on the wrapper."""
+
+    def __init__(self, vae: nn.Module, distri_config: DistriConfig, upcast: bool = False):
         super().__init__()
-        if bool(vae.config.get("force_upcast", False)):
+        if not upcast and bool(vae.config.get("force_upcast", False)):
             raise ValueError("this VAE's config sets force_upcast=True: it overflows in fp16 (the stock SDXL VAE does), and "
-                             "the patch-parallel decode runs in fp16 only.  Use an fp16-safe VAE (SD1.x's, or an fp16-fixed "
-                             "SDXL VAE), or set force_upcast=False in its config at your own risk.")
+                             "the patch-parallel decode runs in fp16 unless upcast=True is passed (vae_upcast=True in the "
+                             "pipelines), which runs the up blocks in fp32 as diffusers does.  Otherwise use an fp16-safe VAE "
+                             "(SD1.x's, or an fp16-fixed SDXL VAE), or set force_upcast=False in its config at your own risk.")
         view = copy.copy(distri_config)
         view.n_device_per_batch = distri_config.world_size       # split_idx() == rank: every world rank is a patch rank
         view.split_batch = False                                 # one patch group: the whole world
@@ -82,15 +111,20 @@ class DistriAutoencoderKLPP(nn.Module):
         self.vae = vae
         self.view = view
         self.distri_config = distri_config
-        install_vae_wrappers(vae.decoder, view)
+        self.upcast = upcast
+        self._config = vae.config
+        if upcast:
+            apply_upcast_split(vae)
+            self._config = type(vae.config)({**vae.config, "force_upcast": False})
+        install_vae_wrappers(vae.decoder, view, upcast=upcast)
         self.comm_manager = None
         self.row_units = None
-        self._shape = None
+        self._layout_key = None
         self.output_buffer = None
 
     @property
     def config(self):
-        return self.vae.config
+        return self._config
 
     @property
     def dtype(self):
@@ -107,9 +141,13 @@ class DistriAutoencoderKLPP(nn.Module):
         z = self.vae.post_quant_conv(z).contiguous(memory_format=torch.channels_last)
         return self.vae.decoder(z)
 
+    def _out_dtype(self):
+        return next(self.vae.decoder.conv_out.parameters()).dtype
+
     def _lay_out(self, z):
         """Row plan, and with more than one rank the decoder's comm manager, for latents of z's shape: one registration pass
-        (the wrappers size their slots; its image is discarded), then the arena.  A new shape replaces the previous arena."""
+        (the wrappers size their slots by the dtypes they see; its image is discarded), then the arena.  A new shape, upcast
+        state or output dtype replaces the previous arena."""
         cfg = self.view
         n = cfg.n_device_per_batch
         b, _, h, w = z.shape
@@ -130,7 +168,7 @@ class DistriAutoencoderKLPP(nn.Module):
                 m._kvmaps = None                 # tensor maps of the old arena
         self.output_buffer = None
         cm = PatchParallelismCommManager(cfg)
-        cm.register_output(b, self.vae.config.out_channels, 8 * h, 8 * w)
+        cm.register_output(b, self.vae.config.out_channels, 8 * h, 8 * w, dtype=self._out_dtype())
         for m in modules:
             m.set_comm_manager(cm)
         self._decode_strip(z)
@@ -146,9 +184,10 @@ class DistriAutoencoderKLPP(nn.Module):
             raise RuntimeError(f"DistriAutoencoderKLPP decodes fp16 CUDA latents only (got {z.dtype} on {z.device})")
         b, _, h, w = z.shape
         units = vae_row_plan(h, n)
-        if tuple(z.shape) != self._shape:
+        key = (tuple(z.shape), self.upcast, self._out_dtype())
+        if key != self._layout_key:
             self._lay_out(z)
-            self._shape = tuple(z.shape)
+            self._layout_key = key
         cm = self.comm_manager
         if cm is not None:
             cm.step_begin(0)
@@ -156,13 +195,14 @@ class DistriAutoencoderKLPP(nn.Module):
         if cm is not None:
             C, H, W = strip.shape[1], 8 * h, 8 * w
             if self.output_buffer is None:
-                self.output_buffer = torch.empty((b, C, H, W), device=z.device, dtype=z.dtype)
+                self.output_buffer = torch.empty((b, C, H, W), device=z.device, dtype=strip.dtype)
             strip = strip.contiguous()
             hs = strip.shape[2]
-            assert tuple(strip.shape) == (b, C, 8 * units[r], W)
-            _lib.check(_lib.lib().df_output_gather_2d(cm.world, strip.data_ptr(), self.output_buffer.data_ptr(), b, C, H, W,
-                                                      b, hs, W, 0, 8 * row_offset(units, r), 0, 0, cm.output_off,
-                                                      torch.cuda.current_stream().cuda_stream), "df_output_gather_2d")
+            assert tuple(strip.shape) == (b, C, 8 * units[r], W) and strip.dtype == self.output_buffer.dtype
+            _lib.check(_lib.lib().df_output_gather_2d_dtype(cm.world, strip.data_ptr(), self.output_buffer.data_ptr(), b, C, H,
+                                                            W, b, hs, W, 0, 8 * row_offset(units, r), 0, 0, cm.output_off,
+                                                            _lib.dtype_code(strip.dtype), torch.cuda.current_stream().cuda_stream),
+                       "df_output_gather_2d_dtype")
             cm.join()
             image = self.output_buffer.clone()
         else:

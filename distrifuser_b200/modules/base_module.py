@@ -47,6 +47,7 @@ class BaseModule(nn.Module):
         self.buffer_list = None
         self.idx = None
         self.row_units = None            # units of latent rows per patch rank (DistriUNetPP's row plan); None: equal strips
+        self.allow_fp32 = False          # True: fp32 tensors are accepted too (the VAE decoder's upcast part)
 
     def forward(self, *args, **kwargs):
         raise NotImplementedError
@@ -75,9 +76,10 @@ class BaseModule(nn.Module):
         cm = self.comm_manager
         return cm is not None and cm.arena is None
 
-    @staticmethod
-    def _require_cuda_half(x: torch.Tensor, who: str):
-        if not (x.is_cuda and x.dtype == torch.float16):
-            raise RuntimeError(
-                f"{who}: distrifuser_b200 runs fp16 tensors on a CUDA device only (got {x.dtype} on {x.device}); "
-                "there is no CPU / eager fallback")
+    def _require_cuda_half(self, x: torch.Tensor, who: str):
+        if x.is_cuda and (x.dtype == torch.float16 or (self.allow_fp32 and x.dtype == torch.float32)):
+            return
+        what = "fp16 or fp32" if self.allow_fp32 else "fp16"
+        raise RuntimeError(
+            f"{who}: distrifuser_b200 runs {what} tensors on a CUDA device only (got {x.dtype} on {x.device}); "
+            "there is no CPU / eager fallback")

@@ -95,14 +95,15 @@ class DistriConv2dPP(BaseModule):
                 st = torch.cuda.current_stream().cuda_stream
                 off, sb = cm.tensor_off[self.idx], cm.slot_bytes[self.idx]
                 sync = cfg.mode == "full_sync" or self._is_sync_step()
+                dt = _lib.dtype_code(x.dtype)                        # fp16, or fp32 in the VAE decoder's upcast part
                 if sync:                                             # conv2d.py:92-93: fresh halos
-                    _lib.check(L.df_halo_push(cm.group, x.data_ptr(), b, h, w, c, self.idx, off, sb, up, down, st),
-                               "df_halo_push")
-                _lib.check(L.df_halo_assemble(cm.group, x.data_ptr(), xp.data_ptr(), b, h, w, c, self.idx, off, sb,
-                                              up, down, 1, st), "df_halo_assemble")
+                    _lib.check(L.df_halo_push_dtype(cm.group, x.data_ptr(), b, h, w, c, self.idx, off, sb, up, down, dt, st),
+                               "df_halo_push_dtype")
+                _lib.check(L.df_halo_assemble_dtype(cm.group, x.data_ptr(), xp.data_ptr(), b, h, w, c, self.idx, off, sb,
+                                                    up, down, 1, dt, st), "df_halo_assemble_dtype")
                 out = self._conv(xp, (0, self.module.padding[1]), residual, fold_bias, bias)   # conv2d.py:95-110
                 if not sync and cfg.mode != "no_sync":               # conv2d.py:111-112: ship for the next step
-                    _lib.check(L.df_halo_push(cm.group, x.data_ptr(), b, h, w, c, self.idx, off, sb, up, down, st),
-                               "df_halo_push")
+                    _lib.check(L.df_halo_push_dtype(cm.group, x.data_ptr(), b, h, w, c, self.idx, off, sb, up, down, dt, st),
+                               "df_halo_push_dtype")
         self.counter += 1
         return out

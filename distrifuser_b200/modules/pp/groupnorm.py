@@ -67,7 +67,8 @@ class DistriGroupNorm(BaseModule):
         else:
             y = torch.empty((b, c, h + 2, w), dtype=x.dtype, device=x.device, memory_format=torch.channels_last)
         L = _lib.lib()
-        nbytes = L.df_groupnorm_scratch_bytes(b, G, h, w, c)
+        dt = _lib.dtype_code(x.dtype)                # fp16, or fp32 in the VAE decoder's upcast part
+        nbytes = L.df_groupnorm_scratch_bytes_dtype(b, G, h, w, c, dt)
         if self._scratch is None or self._scratch.numel() < nbytes:
             self._scratch = torch.zeros(nbytes, dtype=torch.uint8, device=x.device)   # carries a self-resetting ticket
         cm = self.comm_manager
@@ -86,26 +87,26 @@ class DistriGroupNorm(BaseModule):
         apitch = 0
         if addend is not None:
             addend = addend.reshape(b, c)
-            if addend.stride(1) != 1 or addend.stride(0) % 8 != 0 or addend.data_ptr() % 16 != 0:
+            if addend.stride(1) != 1 or addend.stride(0) % (16 // addend.element_size()) != 0 or addend.data_ptr() % 16 != 0:
                 addend = addend.contiguous()
             apitch = addend.stride(0)                 # a column slice of the batched time-embedding projection: no copy
             assert addend.dtype == x.dtype
         st = torch.cuda.current_stream().cuda_stream
         if halo is None:
-            _lib.check(L.df_groupnorm_fwd_weighted(comm, x.data_ptr(), addend.data_ptr() if addend is not None else None, apitch,
-                                                   y.data_ptr(), gamma, beta, b, h, w, c, G, float(module.eps), mode, bessel, neg_fb,
-                                                   int(self.fuse_silu), self.idx or 0, off, sb, mask, weights,
-                                                   self._scratch.data_ptr(), st), "df_groupnorm_fwd_weighted")
+            _lib.check(L.df_groupnorm_fwd_dtype(comm, x.data_ptr(), addend.data_ptr() if addend is not None else None, apitch,
+                                                y.data_ptr(), gamma, beta, b, h, w, c, G, float(module.eps), mode, bessel, neg_fb,
+                                                int(self.fuse_silu), self.idx or 0, off, sb, mask, weights,
+                                                self._scratch.data_ptr(), dt, st), "df_groupnorm_fwd_dtype")
         else:
             h_idx, h_off, h_sb, up, down, push = halo
-            _lib.check(L.df_groupnorm_halo_fwd_weighted(cm.group, x.data_ptr(), addend.data_ptr() if addend is not None else None,
-                                                        apitch, y.data_ptr(), gamma, beta, b, h, w, c, G, float(module.eps), mode,
-                                                        bessel, neg_fb, int(self.fuse_silu), self.idx or 0, off, sb, mask, weights,
-                                                        self._scratch.data_ptr(), h_idx, h_off, h_sb, up, down, int(push), 1, st),
-                       "df_groupnorm_halo_fwd_weighted")
+            _lib.check(L.df_groupnorm_halo_fwd_dtype(cm.group, x.data_ptr(), addend.data_ptr() if addend is not None else None,
+                                                     apitch, y.data_ptr(), gamma, beta, b, h, w, c, G, float(module.eps), mode,
+                                                     bessel, neg_fb, int(self.fuse_silu), self.idx or 0, off, sb, mask, weights,
+                                                     self._scratch.data_ptr(), h_idx, h_off, h_sb, up, down, int(push), 1, dt, st),
+                       "df_groupnorm_halo_fwd_dtype")
         if prof is not None:
             e1.record()
-            prof.append(dict(kernel="groupnorm", kind="gn", flops=0.0, bytes=4.0 * x.numel(), shape=tuple(x.shape),
+            prof.append(dict(kernel="groupnorm", kind="gn", flops=0.0, bytes=2.0 * x.element_size() * x.numel(), shape=tuple(x.shape),
                              start=e0, end=e1))
         self.counter += 1
         return y

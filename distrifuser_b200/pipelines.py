@@ -13,12 +13,23 @@ from .models.naive_patch_sdxl import NaivePatchUNet
 from .utils import DistriConfig, PatchParallelismCommManager
 
 
-def _distribute_vae(pipeline, distri_config: DistriConfig, distributed_vae: bool):
-    """distributed_vae=True: the pipeline's own VAE decodes patch-parallel on every rank (DistriAutoencoderKLPP)."""
+def _pop_vae_kwargs(kwargs) -> tuple[bool, bool]:
+    """(distributed_vae, vae_upcast) of from_pretrained, checked before anything is loaded.  distributed_vae=True: the VAE decode
+    runs split over every rank; vae_upcast=True: ... with its up blocks in fp32 (force_upcast VAEs, e.g. the stock SDXL VAE)."""
+    distributed_vae = kwargs.pop("distributed_vae", False)
+    vae_upcast = kwargs.pop("vae_upcast", False)
+    if vae_upcast and not distributed_vae:
+        raise ValueError("vae_upcast=True applies to the patch-parallel VAE decode: pass distributed_vae=True as well")
+    return distributed_vae, vae_upcast
+
+
+def _distribute_vae(pipeline, distri_config: DistriConfig, distributed_vae: bool, vae_upcast: bool = False):
+    """distributed_vae=True: the pipeline's own VAE decodes patch-parallel on every rank (DistriAutoencoderKLPP); vae_upcast=True
+    runs its up blocks in fp32 (the stock SDXL VAE needs this)."""
     if distributed_vae:
         if getattr(pipeline, "vae", None) is None:
             raise ValueError("distributed_vae=True, but the pipeline has no VAE")
-        pipeline.vae = DistriAutoencoderKLPP(pipeline.vae, distri_config)
+        pipeline.vae = DistriAutoencoderKLPP(pipeline.vae, distri_config, upcast=vae_upcast)
     return pipeline
 
 
@@ -43,13 +54,16 @@ class _DistriPipelineBase:
 
     @classmethod
     def from_synthetic(cls, distri_config: DistriConfig, unet=None, unet_config: dict | None = None, seed: int = 0,
-                       scheduler=None, torch_dtype=torch.float16, controlnet=None, vae=None):
+                       scheduler=None, torch_dtype=torch.float16, controlnet=None, vae=None, vae_upcast: bool = False):
         """Random-weight SDXL / SD1.x UNet (torch default init under manual_seed(seed), SURVEY 8d) + latent pipeline.
         `controlnet`: a compat ControlNetModel run patch-parallel inside every UNet call (the pipeline then takes image=...).
         `vae`: an AutoencoderKL (compat.vae) whose decoder runs patch-parallel on every rank (DistriAutoencoderKLPP); the
-        pipeline then also returns images with output_type="pt"."""
+        pipeline then also returns images with output_type="pt".  `vae_upcast`: its up blocks decode in fp32, as diffusers
+        decodes a force_upcast VAE (DistriAutoencoderKLPP(upcast=True))."""
         from .compat.pipeline import SyntheticLatentPipeline
         from .compat.unet_2d_condition import SD15, SDXL, UNet2DConditionModel
+        if vae_upcast and vae is None:
+            raise ValueError("vae_upcast=True applies to the patch-parallel VAE decode: pass vae= as well")
         if unet is None:
             torch.manual_seed(seed)
             with torch.device(distri_config.device):
@@ -59,7 +73,7 @@ class _DistriPipelineBase:
             controlnet = controlnet.to(distri_config.device, torch_dtype).eval()
         unet = _wrap(unet, distri_config, controlnet)
         if vae is not None:
-            vae = DistriAutoencoderKLPP(vae.to(distri_config.device, torch_dtype).eval(), distri_config)
+            vae = DistriAutoencoderKLPP(vae.to(distri_config.device, torch_dtype).eval(), distri_config, upcast=vae_upcast)
         pipe = SyntheticLatentPipeline(unet, scheduler, sdxl=cls.sdxl, device=distri_config.device, dtype=torch_dtype, vae=vae)
         return cls(pipe, distri_config)
 
@@ -171,11 +185,11 @@ class DistriSDXLPipeline(_DistriPipelineBase):
         device = distri_config.device
         name = kwargs.pop("pretrained_model_name_or_path", "stabilityai/stable-diffusion-xl-base-1.0")
         torch_dtype = kwargs.pop("torch_dtype", torch.float16)
-        distributed_vae = kwargs.pop("distributed_vae", False)      # True: the VAE decode runs split over every rank
+        distributed_vae, vae_upcast = _pop_vae_kwargs(kwargs)
         unet = UNet2DConditionModel.from_pretrained(name, torch_dtype=torch_dtype, subfolder="unet").to(device)
         unet = _wrap(unet, distri_config)
         pipeline = StableDiffusionXLPipeline.from_pretrained(name, torch_dtype=torch_dtype, unet=unet, **kwargs).to(device)
-        pipeline = _distribute_vae(pipeline, distri_config, distributed_vae)
+        pipeline = _distribute_vae(pipeline, distri_config, distributed_vae, vae_upcast)
         return DistriSDXLPipeline(pipeline, distri_config)
 
     def _static_inputs(self, **kwargs):                              # pipelines.py:62-129
@@ -216,11 +230,11 @@ class DistriSDPipeline(_DistriPipelineBase):
         device = distri_config.device
         name = kwargs.pop("pretrained_model_name_or_path", "CompVis/stable-diffusion-v1-4")
         torch_dtype = kwargs.pop("torch_dtype", torch.float16)
-        distributed_vae = kwargs.pop("distributed_vae", False)      # True: the VAE decode runs split over every rank
+        distributed_vae, vae_upcast = _pop_vae_kwargs(kwargs)
         unet = UNet2DConditionModel.from_pretrained(name, torch_dtype=torch_dtype, subfolder="unet").to(device)
         unet = _wrap(unet, distri_config)
         pipeline = StableDiffusionPipeline.from_pretrained(name, torch_dtype=torch_dtype, unet=unet, **kwargs).to(device)
-        pipeline = _distribute_vae(pipeline, distri_config, distributed_vae)
+        pipeline = _distribute_vae(pipeline, distri_config, distributed_vae, vae_upcast)
         return DistriSDPipeline(pipeline, distri_config)
 
     def _static_inputs(self, **kwargs):                              # pipelines.py:219-259

@@ -192,7 +192,7 @@ class PatchParallelismCommManager:
         self.dtypes: list[torch.dtype] = []
         self.tensor_off: list[int] = []
         self.layer_types: list[str] = []
-        self.output_spec = None          # (B, C, H, W) of the final epsilon, registered by DistriUNetPP
+        self.output_spec = None          # (B, C, H, W, element size) of the final epsilon / image, registered by the model
         self.output_off = 0
         self.arena = None                # torch uint8 view of this rank's arena
         self._arena_ptr = None
@@ -225,8 +225,8 @@ class PatchParallelismCommManager:
         self.layer_types.append(layer_type or "")
         return len(self.starts) - 1
 
-    def register_output(self, B: int, Cc: int, H: int, W: int):
-        self.output_spec = (B, Cc, H, W)
+    def register_output(self, B: int, Cc: int, H: int, W: int, dtype: torch.dtype = torch.float16):
+        self.output_spec = (B, Cc, H, W, torch.empty((), dtype=dtype).element_size())
 
     # ------------------------------------------------------------------ arena layout (pure host arithmetic)
     def _layout(self):
@@ -245,8 +245,8 @@ class PatchParallelismCommManager:
             off += n * sb
         self.output_off = off
         if self.output_spec is not None:
-            B, Cc, H, W = self.output_spec
-            off += _align(B * Cc * H * W * 2, 1024)
+            B, Cc, H, W, esize = self.output_spec
+            off += _align(B * Cc * H * W * esize, 1024)
         bank_stride = _align(off - header, 1024)
         return header + NBANKS * bank_stride, bank_stride
 

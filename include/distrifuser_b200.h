@@ -13,7 +13,9 @@
  *   - all pointers are DEVICE pointers unless the name ends in _host; `stream` is a cudaStream_t.
  *   - no entry point synchronises the host or allocates device memory (graph-capturable), except the
  *     df_symm_* / df_tensormap_* set-up calls.
- *   - activations are fp16, NHWC ("channels_last") for 4-D tensors, [b, tokens, C] for sequences.
+ *   - activations are fp16, NHWC ("channels_last") for 4-D tensors, [b, tokens, C] for sequences.  The *_dtype calls
+ *     take the element type (DF_F16 or DF_F32) of the activations, gamma / beta and the addend: fp32 serves the VAE
+ *     decoder's upcast part (its up blocks overflow fp16).
  *
  * Symmetric arena layout (one per rank, mapped into every peer with CUDA IPC):
  *   bank k in [0, DF_NBANKS): byte offset k * bank_stride; inside a bank every registered tensor has
@@ -36,6 +38,8 @@ extern "C" {
 #define DF_IPC_HANDLE_BYTES 64
 #define DF_TENSORMAP_BYTES 128
 #define DF_ZERO_CONV_MAX_PROBLEMS 13   /* zero convs of one ControlNet call: SDXL 10, SD1.x 13 */
+#define DF_F16 0                       /* element types of the *_dtype calls */
+#define DF_F32 1
 
 /* ---- errors / info ------------------------------------------------------------------------------ */
 const char* df_last_error(void);
@@ -131,6 +135,24 @@ int df_groupnorm_halo_fwd_weighted(df_comm_t comm, const void* x, const void* ad
                                    void* scratch, int halo_idx, uint64_t halo_off, uint64_t halo_slot_bytes, int up_rank,
                                    int down_rank, int push, int wait_flags, void* stream);
 
+/* The *_weighted GroupNorm calls for either element type (the calls above are these with DF_F16).  DF_F32 accumulates the
+ * statistics around a shift per (sample, group) -- x + addend at pixel 0 of the sample, the group's first channel -- so that
+ * activations with |mean| >> std (1e5 in the SDXL VAE's up blocks) keep their variance, and its stats slots hold
+ * (mean, biased variance) per member, pooled as var = sum_p w_p (var_p + (mean_p - mean)^2).  DF_F32 takes modes 0 and 1
+ * only.  Scratch: df_groupnorm_scratch_bytes_dtype() (the grid differs with the element size).  Halo slots: 2*b*w*C elements. */
+size_t df_groupnorm_scratch_bytes_dtype(int b, int groups, int h, int w, int C, int dtype);
+int df_groupnorm_fwd_dtype(df_comm_t comm, const void* x, const void* addend, int64_t addend_pitch, void* y, const void* gamma,
+                           const void* beta, int b, int h, int w, int C, int groups, float eps, int mode, int bessel,
+                           int neg_var_fallback, int fuse_silu, int idx, uint64_t tensor_off, uint64_t slot_bytes,
+                           uint32_t group_mask, const int32_t* src_weight_host /* [comm.world] */, void* scratch, int dtype,
+                           void* stream);
+int df_groupnorm_halo_fwd_dtype(df_comm_t comm, const void* x, const void* addend, int64_t addend_pitch, void* y_padded,
+                                const void* gamma, const void* beta, int b, int h, int w, int C, int groups, float eps, int mode,
+                                int bessel, int neg_var_fallback, int fuse_silu, int idx, uint64_t tensor_off,
+                                uint64_t slot_bytes, uint32_t group_mask, const int32_t* src_weight_host /* [comm.world] */,
+                                void* scratch, int halo_idx, uint64_t halo_off, uint64_t halo_slot_bytes, int up_rank,
+                                int down_rank, int push, int wait_flags, int dtype, void* stream);
+
 /* ---- conv halo exchange: replaces the boundary stack + all_gather + cat/pad of DistriConv2dPP.forward
  *      (distrifuser/modules/pp/conv2d.py:72-93).  x: [b,h,w,C] NHWC fp16, one halo row (padding 1).
  *      df_halo_push sends x's first row to patch-neighbour `up_rank` (its bottom halo) and x's last row to
@@ -142,6 +164,12 @@ int df_halo_push(df_comm_t comm, const void* x, int b, int h, int w, int C, int 
 int df_halo_assemble(df_comm_t comm, const void* x, void* xp, int b, int h, int w, int C, int idx,
                      uint64_t tensor_off, uint64_t slot_bytes, int up_rank, int down_rank, int wait_flags,
                      void* stream);
+/* The same two calls for either element type (DF_F16 or DF_F32): rows are copied as bytes, w*C*element size of them. */
+int df_halo_push_dtype(df_comm_t comm, const void* x, int b, int h, int w, int C, int idx, uint64_t tensor_off,
+                       uint64_t slot_bytes, int up_rank, int down_rank, int dtype, void* stream);
+int df_halo_assemble_dtype(df_comm_t comm, const void* x, void* xp, int b, int h, int w, int C, int idx,
+                           uint64_t tensor_off, uint64_t slot_bytes, int up_rank, int down_rank, int wait_flags, int dtype,
+                           void* stream);
 
 /* ---- fused multi-head attention over per-rank K/V segments: replaces torch.cat(full_kv)+split+SDPA of
  *      DistriSelfAttentionPP._forward (distrifuser/modules/pp/attn.py:127-153) and the SDPA of
@@ -204,9 +232,13 @@ int df_output_gather(df_comm_t comm, const void* strip, void* out, int B, int C,
 /* Same gather for a strip that need not span the full width: replaces the all_gather + cat(dim=2 or 3) of
  * NaivePatchUNet.forward (distrifuser/models/naive_patch_sdxl.py:151-154,195-197).  strip: [bs,C,hs,ws] NCHW fp16,
  * placed at batch `batch0`, row `row0`, column `col0` of the [B,C,H,W] image.  16-byte stores when ws, col0 and W are
- * multiples of 8 (or ws == W and hs*W is), 2-byte stores otherwise. */
+ * multiples of 8 (or ws == W and hs*W, row0*W and H*W are), 2-byte stores otherwise. */
 int df_output_gather_2d(df_comm_t comm, const void* strip, void* out, int B, int C, int H, int W, int bs, int hs, int ws,
                         int batch0, int row0, int col0, int idx, uint64_t tensor_off, void* stream);
+/* df_output_gather_2d for either element type (DF_F16 or DF_F32; the arena's output region holds B*C*H*W of them).  16-byte
+ * stores when the runs and their destinations are whole 16-byte vectors (8 halves, 4 floats), element stores otherwise. */
+int df_output_gather_2d_dtype(df_comm_t comm, const void* strip, void* out, int B, int C, int H, int W, int bs, int hs, int ws,
+                              int batch0, int row0, int col0, int idx, uint64_t tensor_off, int dtype, void* stream);
 
 /* ---- fused GEGLU gate of the transformer feed-forward: out[r, c] = in[r, c] * gelu_erf(in[r, cols + c]).
  *      Not one of the reference's wrapped modules (diffusers FeedForward, SURVEY Appendix A) but on the per-step

@@ -4,9 +4,13 @@
                                                   # decoder in fp16 on torch's kernels) and df_attn_wide_fwd vs
                                                   # F.scaled_dot_product_attention at the mid-block shapes
   torchrun --nproc-per-node N tools/bench_vae.py --split   # the product decode split over N GPUs (rank 0 prints)
+  python tools/bench_vae.py --upcast --no-kernel   # the stock SDXL VAE (force_upcast) decoded with upcast=True, against the
+                                                  # compat decoder under diffusers' upcast split (fp16 to the mid block, fp32
+                                                  # after) on torch's kernels; --split works with it too
 
 Every line carries the card's name, power limit and SM clock, read with nvidia-smi in the same run.  Decode times are CUDA
-events around whole decode calls after warm-up (median of --iters); kernel times are CUDA graphs of --launches back-to-back
+events around whole decode calls after warm-up (median of --iters), with torch.cuda.max_memory_allocated of each decode
+(peak_mib; reset before it, so it includes the model's weights); kernel times are CUDA graphs of --launches back-to-back
 launches, TFLOP/s from the shape (4 L^2 d, d = 512)."""
 import argparse
 import json
@@ -44,30 +48,41 @@ def _time(fn, iters, warmup=1):
     return sorted(ts)[len(ts) // 2]
 
 
-def _vae(seed=11):
-    from distrifuser_b200.compat.vae import SD15_VAE, AutoencoderKL
+def _vae(seed=11, upcast=False):
+    from distrifuser_b200.compat.vae import SD15_VAE, SDXL_VAE, AutoencoderKL
     torch.manual_seed(seed)
-    return AutoencoderKL(**SD15_VAE).to("cuda", torch.float16).eval()
+    return AutoencoderKL(**(SDXL_VAE if upcast else SD15_VAE)).to("cuda", torch.float16).eval()
 
 
-def bench_decode(px, iters, split):
-    from distrifuser_b200.models.distri_vae_pp import DistriAutoencoderKLPP
+def _timed(row, key, fn, iters):
+    """row[key + "_ms"] and row[key + "_peak_mib"] of fn, or "out of memory"."""
+    torch.cuda.empty_cache()
+    torch.cuda.reset_peak_memory_stats()
+    try:
+        with torch.no_grad():
+            row[key + "_ms"] = round(_time(fn, iters), 2)
+        row[key + "_peak_mib"] = round(torch.cuda.max_memory_allocated() / 2 ** 20)
+    except torch.cuda.OutOfMemoryError:
+        row[key + "_ms"] = "out of memory"
+    torch.cuda.empty_cache()
+
+
+def bench_decode(px, iters, split, upcast):
+    from distrifuser_b200.models.distri_vae_pp import DistriAutoencoderKLPP, apply_upcast_split
     from distrifuser_b200.utils import DistriConfig
     cfg = DistriConfig(height=px, width=px, split_batch=False)
     z = torch.randn(1, 4, px // 8, px // 8, generator=torch.Generator().manual_seed(5)).to("cuda", torch.float16)
-    pp = DistriAutoencoderKLPP(_vae(), cfg)
-    with torch.no_grad():
-        t_pp = _time(lambda: pp.decode(z), iters)
-    row = dict(what="decode", px=px, world=cfg.world_size, product_ms=round(t_pp, 2))
-    if not split:
-        base = _vae()
-        with torch.no_grad():
-            try:
-                row["torch_fp16_ms"] = round(_time(lambda: base.decode(z), iters), 2)
-            except torch.cuda.OutOfMemoryError:
-                row["torch_fp16_ms"] = "out of memory"
-        del base
+    row = dict(what="decode_upcast" if upcast else "decode", px=px, world=cfg.world_size)
+    pp = DistriAutoencoderKLPP(_vae(upcast=upcast), cfg, upcast=upcast)
+    _timed(row, "product", lambda: pp.decode(z), iters)
     pp.close()
+    del pp
+    if not split:
+        base = _vae(upcast=upcast)
+        if upcast:
+            apply_upcast_split(base)
+        _timed(row, "torch_upcast_split" if upcast else "torch_fp16", lambda: base.decode(z), iters)
+        del base
     torch.cuda.empty_cache()
     return row
 
@@ -122,13 +137,14 @@ def main():
     ap.add_argument("--launches", type=int, default=4)
     ap.add_argument("--split", action="store_true", help="under torchrun: the product decode only, over every rank")
     ap.add_argument("--no-kernel", action="store_true")
+    ap.add_argument("--upcast", action="store_true", help="the SDXL VAE with fp32 up blocks (DistriAutoencoderKLPP(upcast=True))")
     a = ap.parse_args()
     assert torch.cuda.is_available(), "bench_vae measures on a GPU"
     sizes = [int(s) for s in a.sizes.split(",")]
     info = card()
     rank0 = int(os.environ.get("RANK", "0")) == 0
     for px in sizes:
-        row = bench_decode(px, a.iters, a.split)
+        row = bench_decode(px, a.iters, a.split, a.upcast)
         if rank0:
             print(json.dumps(dict(row, card=info)), flush=True)
     if not a.split and not a.no_kernel:
